@@ -83,10 +83,6 @@ extern "C" int fxg_ctx_create(int device, fxg_ctx **out) {
         fxg_set_error("device %d is sm_%d%d; libfxg is built for sm_90a only", device, prop.major, prop.minor);
         return FXG_ENODEV;
     }
-    if (const char *g = getenv("FXG_L2_FETCH")) {            // A/B: L2 fetch granularity (32 / 64 / 128 bytes)
-        const int v = atoi(g);
-        if (v == 32 || v == 64 || v == 128) cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, (size_t)v);
-    }
     fxg_ctx *c = new fxg_ctx();
     c->device = device;
     c->sm_count = prop.multiProcessorCount;
@@ -114,7 +110,7 @@ extern "C" void fxg_ctx_destroy(fxg_ctx *c) {
     }
     for (int i = 0; i < FXG_PROF_SLOTS; ++i)
         for (int j = 0; j < 2; ++j) if (c->prof_ev[i][j]) cudaEventDestroy(c->prof_ev[i][j]);
-    c->tile_desc.release(); c->seg.release(); c->cut.release(); c->row_tmp.release(); c->rows.release();
+    c->tile_desc.release(); c->seg.release(); c->row_tmp.release(); c->rows.release();
     c->counters.release(); c->params.release(); c->plan.release(); c->misc.release(); c->stage_file.release();
     if (c->own_stream && c->stream) cudaStreamDestroy(c->stream);
     delete c;

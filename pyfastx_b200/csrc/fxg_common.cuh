@@ -67,7 +67,7 @@ struct fxg_ctx {
     void        *ring = nullptr;         // pinned ring of the path stager (32 x 16 MiB), one event per slot
     cudaEvent_t  ring_ev[32] = {};
     // scan scratch
-    FxgScratch   tile_desc, seg, cut, row_tmp, rows, counters, params, plan, misc, stage_file;
+    FxgScratch   tile_desc, seg, row_tmp, rows, counters, params, plan, misc, stage_file;
     void        *h_counters = nullptr;   // pinned, small
     void        *h_one = nullptr;        // pinned + mapped: output of single-query launches (fxg_extract_one_host)
     // single-query service (resident kernel fed through mapped host memory)
@@ -140,9 +140,6 @@ __device__ __forceinline__ void tma_load_1d(void *smem_dst, const void *gsrc, ui
                      smem_u32(smem_dst)),
                  "l"(gsrc), "r"(bytes), "r"(smem_u32(bar))
                  : "memory");
-}
-__device__ __forceinline__ void fence_proxy_async() {
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 
 // 0x80 in every byte of w that equals `c` (c < 0x80).  Exact, 3 ALU ops when the constants

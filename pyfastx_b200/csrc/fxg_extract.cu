@@ -8,12 +8,15 @@
 //   gc_content counting loop    (src/sequence.c:607-631)  A/C/G/T counters (fused, optional)
 // and for FASTQ  pyfastx_read_random_reader (src/read.c:37-45): raw copies of rlen bytes.
 //
-// One warp serves one query.  The covering byte range is streamed in 512-byte rounds
-// (32 lanes x 16 B, 16-byte aligned loads); a warp prefix sum of per-lane kept-byte counts
-// gives every kept byte its rank ("strip" semantics, exact also for records with an odd
-// line); kept bytes are transformed (toupper / complement LUT) and staged in shared memory
-// at their output position (mirrored for reverse strands), then flushed with aligned
-// 16-byte stores; only the ragged first/last words of a round use byte stores.
+// A batch of queries goes to extract_bulk_kernel: a warp owns up to 32 queries, and for records with
+// uniform lines the covering source bytes of every 1 KiB output piece arrive in shared memory by one
+// TMA bulk copy, from which every lane assembles aligned 16-byte output words (slice formula).
+// Every other query -- norm = 0 records, odd lines, short or raw queries, a failed layout check --
+// is served by one whole warp (serve_query_warp): the uniform-line pull path (pull_one) where it
+// applies, else the general strip path (gather_one), which streams the covering byte range in
+// 512-byte rounds and ranks the kept bytes with a warp prefix sum ("strip" semantics, exact also
+// for records with an odd line).  A single query (extract_one_kernel, extract_service_kernel) and
+// FASTQ reads (reads_kernel, read_one_kernel) use the same per-warp code.
 #include "fxg_common.cuh"
 #include <stdlib.h>
 #include <string.h>
@@ -382,62 +385,9 @@ __device__ void serve_query_warp(const uint8_t *__restrict__ file, int64_t fsize
     }
 }
 
-// One warp per query (used when per-query A/C/G/T counts are requested).
-template <bool WANT_ACGT>
-__global__ void __launch_bounds__(XTHREADS, 3) extract_kernel(
-    const uint8_t *__restrict__ file, int64_t fsize, int64_t capacity, const fxg_fasta_row *__restrict__ rows,
-    int64_t n_rows, const int64_t *__restrict__ q_row, const int64_t *__restrict__ q_s,
-    const int64_t *__restrict__ q_e, const int32_t *__restrict__ q_flags, int64_t nq,
-    const int64_t *__restrict__ out_off, uint8_t *__restrict__ out, int64_t *__restrict__ acgt) {
-    __shared__ uint8_t s_lut[3][256];
-    __shared__ __align__(16) uint8_t s_stage[XWARPS][XSTAGE];
-    init_luts(s_lut);
-    __syncthreads();
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int64_t nwarps = (int64_t)gridDim.x * XWARPS;
-    // software pipeline over queries: descriptors are fetched two queries ahead, index rows one
-    // ahead, so the dependent chain  query -> row -> file bytes  is off the critical path
-    struct Desc { int64_t rid, s, e, off; int flags; };
-    auto load_desc = [&](int64_t qq) -> Desc {
-        Desc d; d.rid = -1; d.s = 0; d.e = 0; d.off = 0; d.flags = 0;
-        if (qq < nq) { d.rid = q_row[qq]; d.s = q_s[qq]; d.e = q_e[qq]; d.off = out_off[qq]; d.flags = q_flags ? q_flags[qq] : 0; }
-        return d;
-    };
-    union RowU { fxg_fasta_row r; uint4 v[3]; };
-    auto load_row = [&](int64_t rid) -> RowU {
-        RowU u;
-        u.v[0] = u.v[1] = u.v[2] = make_uint4(0, 0, 0, 0);
-        if (rid >= 0 && rid < n_rows) {
-            const uint4 *p4 = reinterpret_cast<const uint4 *>(rows + rid);
-            u.v[0] = p4[0]; u.v[1] = p4[1]; u.v[2] = p4[2];
-        }
-        return u;
-    };
-    int64_t q = (int64_t)blockIdx.x * XWARPS + warp;
-    Desc d0 = load_desc(q), d1 = load_desc(q + nwarps);
-    RowU r0 = load_row(d0.rid);
-    for (; q < nq; q += nwarps) {
-        const Desc d2 = load_desc(q + 2 * nwarps);
-        const RowU r1 = load_row(d1.rid);
-        serve_query_warp<WANT_ACGT>(file, fsize, capacity, r0.r, d0.rid >= 0 && d0.rid < n_rows, d0.s, d0.e, d0.flags,
-                                    out + d0.off, s_lut, s_stage[warp], lane, WANT_ACGT ? acgt + 4 * q : nullptr);
-        d0 = d1; d1 = d2; r0 = r1;
-    }
-}
-
-// ---- eight lanes per query ---------------------------------------------------------------------------
-// The per-query bookkeeping of the pull path (descriptor, index row, slice -> byte-range arithmetic) is
-// warp-uniform work when a warp serves one query; with a query per 8-lane group the same instructions
-// serve four queries, and every lane still assembles whole aligned 16-byte output words.
-#ifndef FXG_QG
-#define FXG_QG 4
-#endif
-constexpr int QG = FXG_QG;            // lanes per query
-constexpr int QPW = 32 / QG;          // queries per warp and step
-#ifndef FXG_XU
-#define FXG_XU 4
-#endif
-constexpr int XU = FXG_XU;            // output words per lane and step
+// ---- uniform-line output words ----------------------------------------------------------------------------
+// Helpers of the bulk kernel below: the 16-byte transform of kept bytes, and the assembly of any 16 output bytes of a
+// query on uniform lines straight from the file (the ragged first / last word of a query).
 
 // Complement of four bytes at once for the letters that make up almost all nucleotide data: A C G T N in either
 // case.  (b >> 1) & 7 is a perfect hash of these five letters (A 0, C 1, T 2, G 3, N 7), so ONE byte-permute
@@ -530,7 +480,8 @@ __device__ __forceinline__ bool ow_finish(const uint32_t W[6], const WordReq &q,
             V[i] = (V[i] & ~m) | (e2 & m);
         }
     }
-    // conservative layout check: every kept byte must lie in 0x40..0x7f (letters); see ow_finish_line
+    // conservative layout check: every kept byte must be a letter-range byte (>= 0x40, < 0x80); anything else --
+    // which includes the strippable 10 / 13 / 32 -- sends the query to the general strip path
     const uint32_t all = V[0] & V[1] & V[2] & V[3], hi = V[0] | V[1] | V[2] | V[3];
     ok = ok && (all & 0x40404040u) == 0x40404040u && (hi & 0x80808080u) == 0u;
     xform16(V, upper, comp, s_lut);
@@ -541,160 +492,22 @@ __device__ __forceinline__ bool ow_finish(const uint32_t W[6], const WordReq &q,
     return ok;
 }
 
-// 16 output bytes that lie on ONE source line (no line break inside): five aligned words cover them.
-__device__ __forceinline__ bool ow_finish_line(const uint32_t W[5], int o1, bool rev, bool upper, bool comp,
-                                               const uint8_t (*__restrict__ s_lut)[256], uint32_t o[4]) {
-    uint32_t V[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) V[i] = __funnelshift_r(W[i], W[i + 1], o1 * 8);
-    // conservative layout check: every kept byte must be a letter-range byte (>= 0x40, < 0x80); anything else --
-    // which includes the strippable 10 / 13 / 32 -- sends the query to the general strip path
-    const uint32_t hi = V[0] | V[1] | V[2] | V[3];
-    const uint32_t all = V[0] & V[1] & V[2] & V[3];
-    bool ok = (all & 0x40404040u) == 0x40404040u && (hi & 0x80808080u) == 0u;
-    xform16(V, upper, comp, s_lut);
-    if (rev) {
-        o[0] = __byte_perm(V[3], 0, 0x0123); o[1] = __byte_perm(V[2], 0, 0x0123);
-        o[2] = __byte_perm(V[1], 0, 0x0123); o[3] = __byte_perm(V[0], 0, 0x0123);
-    } else { o[0] = V[0]; o[1] = V[1]; o[2] = V[2]; o[3] = V[3]; }
-    return ok;
-}
-
-__global__ void __launch_bounds__(XTHREADS, 3) extract_group_kernel(
-    const uint8_t *__restrict__ file, int64_t fsize, int64_t capacity, const fxg_fasta_row *__restrict__ rows,
-    int64_t n_rows, const int64_t *__restrict__ q_row, const int64_t *__restrict__ q_s,
-    const int64_t *__restrict__ q_e, const int32_t *__restrict__ q_flags, int64_t nq,
-    const int64_t *__restrict__ out_off, uint8_t *__restrict__ out) {
-    __shared__ uint8_t s_lut[3][256];
-    __shared__ __align__(16) uint8_t s_stage[XWARPS][XSTAGE];
-    init_luts(s_lut);
-    __syncthreads();
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int grp = lane / QG, li = lane % QG;
-    const int64_t step = (int64_t)gridDim.x * XWARPS * QPW;
-    for (int64_t qb = ((int64_t)blockIdx.x * XWARPS + warp) * QPW; qb < nq; qb += step) {
-        const int64_t q = qb + grp;
-        const bool valid = q < nq;
-        int64_t rid = -1, s = 0, e = 0, off = 0;
-        int flags = 0;
-        if (valid) { rid = q_row[q]; s = q_s[q]; e = q_e[q]; off = out_off[q]; flags = q_flags ? q_flags[q] : 0; }
-        const bool row_ok = rid >= 0 && rid < n_rows;
-        union RowU { fxg_fasta_row r; uint4 v[3]; } ru;
-        ru.v[0] = ru.v[1] = ru.v[2] = make_uint4(0, 0, 0, 0);
-        if (row_ok) {
-            const uint4 *p4 = reinterpret_cast<const uint4 *>(rows + rid);
-            ru.v[0] = p4[0]; ru.v[1] = p4[1]; ru.v[2] = p4[2];
-        }
-        const fxg_fasta_row &r = ru.r;
-        const int64_t out_len64 = e > s ? e - s : 0;
-        const int64_t bpl64 = r.llen - (int64_t)r.elen;
-        const bool fast = row_ok && out_len64 >= 16 && out_len64 < (1ll << 30) && r.norm && (r.pad[0] & 1) != 0 &&
-                          bpl64 >= 16 && bpl64 < (1ll << 30) && s >= 0 && s < (1ll << 32) && e <= r.slen &&
-                          r.boff >= 0 && r.boff + r.blen + 32 <= capacity && !(flags & FXG_X_RAW);
-        bool bad = false;
-        if (fast) {
-            const uint32_t bpl = (uint32_t)bpl64, out_len = (uint32_t)out_len64;
-            const int elen = (int)r.elen;
-            const uint32_t q_s32 = (uint32_t)s / bpl, rem_s = (uint32_t)s - q_s32 * bpl;
-            const uint32_t inv = (uint32_t)(0x100000000ull / bpl);
-            const uint8_t *fq = file + r.boff + s + (int64_t)elen * (int64_t)q_s32;
-            const bool rev = (flags & FXG_X_REVERSE) != 0;
-            const bool upper = (flags & FXG_X_UPPER) != 0, comp = (flags & FXG_X_COMPLEMENT) != 0;
-            uint8_t *dst = out + off;
-            const uint32_t a = (uint32_t)(reinterpret_cast<uintptr_t>(dst) & 15);
-            const uint32_t total = a + out_len;
-            const uint32_t nwords = (total + 15u) >> 4, hi_last = total & 15u;
-            const uint32_t w_begin = a ? 1u : 0u, w_end = nwords - (hi_last ? 1u : 0u);
-            uint8_t *dst0 = dst - a;                                     // 16-byte aligned
-            // interior words: all 16 slots belong to the query
-            // (XU words per lane and step: 6 * XU loads in flight)
-            for (uint32_t w = w_begin + (uint32_t)li; w < w_end; w += XU * QG) {
-                WordReq rq[XU];
-                uint32_t WW[XU][6], o[4];
-#pragma unroll
-                for (int u = 0; u < XU; ++u) {
-                    const uint32_t wu = w + u * QG;
-                    rq[u] = ow_locate(fq, rem_s, bpl, inv, elen, out_len, rev, 16u * (wu < w_end ? wu : w) - a);
-                }
-#pragma unroll
-                for (int u = 0; u < XU; ++u) ow_load(rq[u], WW[u]);
-#pragma unroll
-                for (int u = 0; u < XU; ++u) {
-                    const uint32_t wu = w + u * QG;
-                    if (u == 0 || wu < w_end) {
-                        if (!ow_finish(WW[u], rq[u], elen, rev, upper, comp, s_lut, o)) bad = true;
-                        *reinterpret_cast<uint4 *>(dst0 + 16u * wu) = make_uint4(o[0], o[1], o[2], o[3]);
-                    }
-                }
-            }
-            // ragged first / last word: take the nearest complete 16 output bytes and shift them into place
-            const bool first = li == 0;
-            if (li < 2 && (first ? a != 0u : hi_last != 0u)) {
-                uint32_t o[4], WE[6];
-                const WordReq re = ow_locate(fq, rem_s, bpl, inv, elen, out_len, rev, first ? 0u : out_len - 16u);
-                ow_load(re, WE);
-                if (!ow_finish(WE, re, elen, rev, upper, comp, s_lut, o)) bad = true;
-                uint64_t lo = (uint64_t)o[0] | ((uint64_t)o[1] << 32), hi = (uint64_t)o[2] | ((uint64_t)o[3] << 32);
-                uint32_t b_lo, b_hi;                                     // slots [b_lo, b_hi) of the word are ours
-                uint8_t *gw;
-                if (first) {
-                    const uint32_t sh = 8u * a;                          // outputs 0.. move up to slot a
-                    if (sh < 64u) { hi = (hi << sh) | (lo >> (64u - sh)); lo <<= sh; } else { hi = lo << (sh - 64u); lo = 0; }
-                    b_lo = a; b_hi = 16u; gw = dst0;
-                } else {
-                    const uint32_t sh = 8u * (16u - hi_last);            // the last hi_last outputs move down to slot 0
-                    if (sh < 64u) { lo = (lo >> sh) | (hi << (64u - sh)); hi >>= sh; } else { lo = hi >> (sh - 64u); hi = 0; }
-                    b_lo = 0u; b_hi = hi_last; gw = dst0 + 16u * (nwords - 1u);
-                }
-                const uint32_t x[4] = {(uint32_t)lo, (uint32_t)(lo >> 32), (uint32_t)hi, (uint32_t)(hi >> 32)};
-#pragma unroll
-                for (uint32_t i = 0; i < 4; ++i) {
-                    const uint32_t b0 = 4u * i;
-                    if (b_lo <= b0 && b0 + 4u <= b_hi) *reinterpret_cast<uint32_t *>(gw + b0) = x[i];
-                    else {
-#pragma unroll
-                        for (uint32_t b = 0; b < 4; ++b)
-                            if (b0 + b >= b_lo && b0 + b < b_hi) gw[b0 + b] = (uint8_t)(x[i] >> (8u * b));
-                    }
-                }
-            }
-        }
-        // queries the group path could not serve (or that failed its layout check): whole warp, one at a time
-        const uint32_t badm = __ballot_sync(0xffffffffu, bad);
-        const bool group_bad = ((badm >> (grp * QG)) & ((1u << QG) - 1u)) != 0;
-        uint32_t fb = __ballot_sync(0xffffffffu, li == 0 && valid && out_len64 > 0 && (!fast || group_bad));
-        while (fb) {
-            const int src = __ffs(fb) - 1;
-            fb &= fb - 1;
-            const int64_t b_rid = shfl_i64(rid, src), b_s = shfl_i64(s, src), b_e = shfl_i64(e, src), b_off = shfl_i64(off, src);
-            const int b_flags = __shfl_sync(0xffffffffu, flags, src);
-            const bool b_ok = b_rid >= 0 && b_rid < n_rows;
-            RowU bu;
-            bu.v[0] = bu.v[1] = bu.v[2] = make_uint4(0, 0, 0, 0);
-            if (b_ok) {
-                const uint4 *p4 = reinterpret_cast<const uint4 *>(rows + b_rid);
-                bu.v[0] = p4[0]; bu.v[1] = p4[1]; bu.v[2] = p4[2];
-            }
-            serve_query_warp<false>(file, fsize, capacity, bu.r, b_ok, b_s, b_e, b_flags, out + b_off, s_lut, s_stage[warp],
-                                    lane, nullptr);
-        }
-    }
-}
-
 // ---- bulk-copy pull path: the covering source range of every 1 KiB output piece travels global -> shared memory
 //      as ONE 1-D TMA bulk copy (cp.async.bulk, completion counted on an mbarrier), several pieces in flight per warp ----
-// In the 4-lanes-per-query kernel the L1 data pipe was the limiter (six 4-byte loads per 16 output bytes, each
-// touching eight different cache lines for the eight queries of a warp), not DRAM.  Here the file bytes never pass through the load/store
-// unit as global loads: the TMA engine writes them to shared memory, every lane assembles its aligned 16-byte output
-// words from three 8-byte shared-memory loads, and a warp's stores are 512 contiguous bytes.
+// Assembling output words from global loads makes the L1 data pipe the limiter (six 4-byte loads per 16 output bytes,
+// each touching a different cache line per query), not DRAM (DESIGN.md section 4).  Here the file bytes
+// never pass through the load/store unit as global loads: the TMA engine writes them to shared memory, every lane
+// assembles its aligned 16-byte output words from three 8-byte shared-memory loads, and a warp's stores are 512
+// contiguous bytes.
 //   * a warp owns a batch of `bq` queries (one per lane: descriptor + index row in registers, the constants the
 //     consumers need in shared memory);
 //   * a query is cut into items of BK_WORDS aligned output words; the items of the batch are enumerated in order by
 //     two warp-uniform cursors (issue / consume) and run through a ring of BK_NS slots per warp: the lane that owns the
 //     query computes the covering, 16-byte aligned source range (slice formula, sequence.c:498-510) and issues the
 //     bulk copy; all lanes consume;
-//   * the layout assumption is verified on every word exactly as in the group kernel; failures and queries that do not
-//     qualify (norm = 0, odd lines, < 16 bytes, RAW ...) are redone by the general strip path.
+//   * the layout assumption is verified on every word (every kept byte in 0x40..0x7f, '\r' where a CRLF break is
+//     expected); failures and queries that do not qualify (norm = 0, odd lines, < 16 bytes, RAW ...) are redone by
+//     serve_query_warp (the per-warp pull path, else the general strip path), one query per warp at a time.
 #ifndef FXG_BK_NS
 #define FXG_BK_NS 4
 #endif
@@ -819,9 +632,6 @@ __global__ void __launch_bounds__(XTHREADS, 3) extract_bulk_kernel(
                 uint32_t bytes = bytes_first;
                 if (pi > 0) item_range(pi, g0, bytes);
                 g0s[slot] = g0;
-#if FXG_BK_FENCE
-                fence_proxy_async();
-#endif
                 mbar_expect_tx(&bars[slot], bytes);
                 tma_load_1d(slots + (size_t)slot * BK_SLOT, fq + g0, bytes, &bars[slot]);
             }
@@ -1363,52 +1173,33 @@ extern "C" int fxg_extract_dev(fxg_ctx *ctx, const fxg_file *f, const fxg_fasta_
     if (nq == 0) return FXG_OK;
     FXG_CHECK_ARG(d_rows && d_row_id && d_s && d_e && d_out_off && d_out, "null device pointer");
     FXG_CUDA(cudaSetDevice(ctx->device));
-    const int grid = gather_grid(ctx, nq);
-    // A/B switches: FXG_EXTRACT_PATH = bulk (default) | group | warp
-    const char *path_env = getenv("FXG_EXTRACT_PATH");
-    const bool want_group = path_env && !strcmp(path_env, "group");
-    const bool want_warp = (path_env && !strcmp(path_env, "warp")) || getenv("FXG_EXTRACT_WARP_PER_QUERY");
     FxgProfScope prof(ctx, FXG_PROF_GATHER);
-    if (!want_warp && !(want_group && !d_acgt)) {
-        static int ctas_per_sm[2] = {0, 0};                 // [with counts]
-        const int v = d_acgt ? 1 : 0;
-        if (!ctas_per_sm[v]) {
-            int nb = 0;
-            if (v) {
-                FXG_CUDA(cudaFuncSetAttribute(extract_bulk_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BK_SMEM));
-                FXG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, extract_bulk_kernel<true>, XTHREADS, BK_SMEM));
-            } else {
-                FXG_CUDA(cudaFuncSetAttribute(extract_bulk_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BK_SMEM));
-                FXG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, extract_bulk_kernel<false>, XTHREADS, BK_SMEM));
-            }
-            ctas_per_sm[v] = nb > 0 ? nb : 1;
+    static int ctas_per_sm[2] = {0, 0};                     // [with counts]
+    const int v = d_acgt ? 1 : 0;
+    if (!ctas_per_sm[v]) {
+        int nb = 0;
+        if (v) {
+            FXG_CUDA(cudaFuncSetAttribute(extract_bulk_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BK_SMEM));
+            FXG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, extract_bulk_kernel<true>, XTHREADS, BK_SMEM));
+        } else {
+            FXG_CUDA(cudaFuncSetAttribute(extract_bulk_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BK_SMEM));
+            FXG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, extract_bulk_kernel<false>, XTHREADS, BK_SMEM));
         }
-        const int64_t resident_warps = (int64_t)ctx->sm_count * ctas_per_sm[v] * XWARPS;
-        // queries per warp batch: a lane per query when there is enough work to fill the machine that way
-        int bq = nq >= resident_warps * 32 ? 32 : (nq >= resident_warps * 16 ? 16 : 8);
-        if (const char *b = getenv("FXG_BK_BQ")) { const int v = atoi(b); if (v >= 1 && v <= 32) bq = v; }   // tests: force a batch width
-        int64_t blocks = (nq + (int64_t)XWARPS * bq - 1) / ((int64_t)XWARPS * bq);
-        const int64_t maxb = (int64_t)ctx->sm_count * ctas_per_sm[v];
-        if (blocks > maxb) blocks = maxb;
-        if (v)
-            extract_bulk_kernel<true><<<(unsigned)blocks, XTHREADS, BK_SMEM, ctx->stream>>>(
-                f->d, f->size, f->capacity, d_rows, n_rows, d_row_id, d_s, d_e, d_flags, nq, d_out_off, d_out, d_acgt, bq);
-        else
-            extract_bulk_kernel<false><<<(unsigned)blocks, XTHREADS, BK_SMEM, ctx->stream>>>(
-                f->d, f->size, f->capacity, d_rows, n_rows, d_row_id, d_s, d_e, d_flags, nq, d_out_off, d_out, nullptr, bq);
-    } else if (d_acgt)
-        extract_kernel<true><<<grid, XTHREADS, 0, ctx->stream>>>(f->d, f->size, f->capacity, d_rows, n_rows, d_row_id, d_s, d_e,
-                                                                d_flags, nq, d_out_off, d_out, d_acgt);
-    else if (want_warp)          // A/B and debugging
-        extract_kernel<false><<<grid, XTHREADS, 0, ctx->stream>>>(f->d, f->size, f->capacity, d_rows, n_rows, d_row_id, d_s, d_e,
-                                                                 d_flags, nq, d_out_off, d_out, nullptr);
-    else {
-        int64_t blocks = (nq + XWARPS * QPW - 1) / (XWARPS * QPW);
-        const int64_t maxb = (int64_t)ctx->sm_count * 6;
-        if (blocks > maxb) blocks = maxb;
-        extract_group_kernel<<<(unsigned)blocks, XTHREADS, 0, ctx->stream>>>(f->d, f->size, f->capacity, d_rows, n_rows, d_row_id,
-                                                                            d_s, d_e, d_flags, nq, d_out_off, d_out);
+        ctas_per_sm[v] = nb > 0 ? nb : 1;
     }
+    const int64_t resident_warps = (int64_t)ctx->sm_count * ctas_per_sm[v] * XWARPS;
+    // queries per warp batch: a lane per query when there is enough work to fill the machine that way
+    int bq = nq >= resident_warps * 32 ? 32 : (nq >= resident_warps * 16 ? 16 : 8);
+    if (const char *b = getenv("FXG_BK_BQ")) { const int v = atoi(b); if (v >= 1 && v <= 32) bq = v; }   // tests: force a batch width
+    int64_t blocks = (nq + (int64_t)XWARPS * bq - 1) / ((int64_t)XWARPS * bq);
+    const int64_t maxb = (int64_t)ctx->sm_count * ctas_per_sm[v];
+    if (blocks > maxb) blocks = maxb;
+    if (v)
+        extract_bulk_kernel<true><<<(unsigned)blocks, XTHREADS, BK_SMEM, ctx->stream>>>(
+            f->d, f->size, f->capacity, d_rows, n_rows, d_row_id, d_s, d_e, d_flags, nq, d_out_off, d_out, d_acgt, bq);
+    else
+        extract_bulk_kernel<false><<<(unsigned)blocks, XTHREADS, BK_SMEM, ctx->stream>>>(
+            f->d, f->size, f->capacity, d_rows, n_rows, d_row_id, d_s, d_e, d_flags, nq, d_out_off, d_out, nullptr, bq);
     FXG_CUDA(cudaGetLastError());
     return FXG_OK;
 }

@@ -1,4 +1,4 @@
-// fxg_inflate.cu -- K6: BGZF member-parallel DEFLATE decoding on the GPU (sm_90a).
+// fxg_inflate.cu -- K6: DEFLATE decoding on the GPU (sm_90a), for BGZF members and for plain gzip from checkpoints.
 //
 // Replaces, for block-gzipped inputs, the reference's zlib read side: gzread during the index scan
 // (src/kseq.c:70) and zran_seek + zran_read per random access (src/index.c:685-686,
@@ -7,12 +7,12 @@
 //   * the host walks the member headers (no inflation) and gets, per member, the compressed range
 //     and -- from the ISIZE trailer -- the uncompressed offset: this is the checkpoint table that
 //     zran would have to inflate the whole file for (src/index.c:381-387);
-//   * one WARP per member inflates it straight into its slot of the uncompressed HBM buffer;
+//   * one THREAD per member inflates it straight into its slot of the uncompressed HBM buffer
+//     (inflate_thread_kernel, with the fxi::Decoder of fxg_inflate_core.cuh);
+//   * crc_members_kernel checks every member's output against its gzip trailer;
 //   * the K1/K2 scans and K3/K5 gathers then run on that buffer exactly as for plain files.
-// Lane 0 runs the (inherently serial) Huffman symbol loop with 10-bit / 9-bit primary lookup tables
-// in shared memory built by all lanes; LZ77 matches are copied by the whole warp.
-// Plain (non-BGZF) gzip streams are not handled here (no independent entry points without a
-// previous serial pass); the host layer inflates those while staging.
+// A plain (non-BGZF) gzip stream has no independent entry points until one serial pass has recorded
+// checkpoints (csrc/fxg_gzip.cpp); with those, inflate_points_kernel decodes a segment per thread.
 #include "fxg_common.cuh"
 #include <zlib.h>
 #include <vector>
@@ -22,389 +22,9 @@
 
 namespace fxg {
 
-constexpr int SHORT_MATCH = 24;        // matches up to this length are copied by the decoding lane itself
-constexpr int IW = 6;                 // warps (members in flight) per CTA
-constexpr int LIT_BITS = 10, DIST_BITS = 9;
-
-struct __align__(8) WarpTables {
-    uint32_t lit[1 << LIT_BITS];      // low half: (len << 9) | symbol, 0 = code longer than LIT_BITS;
-                                      // high half (TWO_LIT set): a second literal decodable from the same bits:
-                                      // TWO_LIT | total length << 24 | second symbol << 16
-    uint16_t dist[1 << DIST_BITS];    // (len << 5) | symbol
-    uint16_t litcnt[16], litsym[288];     // canonical tables for the slow path (long codes)
-    uint16_t distcnt[16], distsym[32];
-    uint8_t  lens[320];
-};
-
-constexpr uint32_t TWO_LIT = 1u << 31;
-
-struct BitReader {
-    const uint8_t *in;
-    int64_t pos, end;      // next byte to load / one past the member's deflate data
-    int64_t lim;           // readable bytes at `in` (whole compressed buffer)
-    uint64_t buf;
-    int nbits;
-    // at least 32 valid bits afterwards: one unaligned 32-bit fetch (two aligned words + funnel shift).
-    // Bytes past `end` are whatever follows in the buffer (trailer, next header); overrun() catches a
-    // stream that really consumes them.
-    __device__ __forceinline__ void refill32() {
-        if (nbits < 32) {
-            if (pos + 8 <= lim) {
-                const uint32_t *w = reinterpret_cast<const uint32_t *>(in + (pos & ~(int64_t)3));
-                const uint32_t v = __funnelshift_r(__ldg(w), __ldg(w + 1), (int)(pos & 3) * 8);
-                buf |= (uint64_t)v << nbits;
-                nbits += 32;
-                pos += 4;
-            } else refill();
-        }
-    }
-    __device__ __forceinline__ void refill() {
-        while (nbits <= 56) {
-            const uint64_t b = pos < end ? in[pos] : 0;
-            ++pos;
-            buf |= b << nbits;
-            nbits += 8;
-        }
-    }
-    __device__ __forceinline__ uint32_t peek(int n) const { return (uint32_t)(buf & ((1ull << n) - 1)); }
-    __device__ __forceinline__ void drop(int n) { buf >>= n; nbits -= n; }
-    __device__ __forceinline__ uint32_t get(int n) { refill(); const uint32_t v = peek(n); drop(n); return v; }
-    __device__ __forceinline__ bool overrun() const { return pos - (nbits >> 3) > end; }
-};
-
-__device__ __forceinline__ uint32_t bitrev(uint32_t v, int n) { return __brev(v) >> (32 - n); }
-
-// canonical slow decode (one bit at a time) -- only for codes longer than the primary table
-__device__ int slow_decode(BitReader &br, const uint16_t *cnt, const uint16_t *sym) {
-    int code = 0, first = 0, index = 0;
-    for (int len = 1; len <= 15; ++len) {
-        code |= (int)br.get(1);
-        const int count = cnt[len];
-        if (code - count < first) return sym[index + (code - first)];
-        index += count;
-        first += count;
-        first <<= 1;
-        code <<= 1;
-    }
-    return -1;
-}
-
-// Build primary + canonical tables for `n` symbols with code lengths lens[0..n) (all lanes).
-// Returns false on an over-subscribed code.
-template <typename E>
-__device__ bool build_table(const uint8_t *lens, int n, E *tab, int tab_bits, int sym_shift, uint16_t *cnt,
-                            uint16_t *sym, int lane) {
-    // counts / offsets by lane 0 (n <= 288)
-    int ok = 1;
-    if (lane == 0) {
-        for (int i = 0; i < 16; ++i) cnt[i] = 0;
-        for (int i = 0; i < n; ++i) cnt[lens[i]]++;
-        int left = 1;
-        for (int len = 1; len <= 15; ++len) {
-            left <<= 1;
-            left -= cnt[len];
-            if (left < 0) ok = 0;
-        }
-        int offs[16];
-        offs[1] = 0;
-        for (int len = 1; len < 15; ++len) offs[len + 1] = offs[len] + cnt[len];
-        for (int i = 0; i < n; ++i)
-            if (lens[i]) sym[offs[lens[i]]++] = (uint16_t)i;
-    }
-    ok = __shfl_sync(0xffffffffu, ok, 0);
-    __syncwarp();
-    for (int i = lane; i < (1 << tab_bits); i += 32) tab[i] = 0;
-    __syncwarp();
-    // canonical codes: first code of each length
-    int next[16];
-    {
-        int code = 0;
-        next[0] = 0;
-        const int c0 = cnt[0];
-        (void)c0;
-        for (int len = 1; len <= 15; ++len) {
-            code = (code + (len > 1 ? cnt[len - 1] : 0)) << 1;
-            next[len] = code;
-        }
-    }
-    // symbols are stored in `sym` grouped by length in increasing symbol order: entry k of length len has
-    // code next[len] + k
-    int base = 0;
-    for (int len = 1; len <= tab_bits; ++len) {
-        const int c = cnt[len];
-        for (int k = lane; k < c; k += 32) {
-            const int s = sym[base + k];
-            const uint32_t code = (uint32_t)(next[len] + k);
-            const uint32_t r = bitrev(code, len);
-            const E e = (E)((len << sym_shift) | s);
-            for (uint32_t j = r; j < (1u << tab_bits); j += (1u << len)) tab[j] = e;
-        }
-        base += c;
-    }
-    __syncwarp();
-    return ok != 0;
-}
-
-__constant__ uint16_t LEN_BASE[29] = {3, 4, 5, 6, 7, 8, 9, 10, 11, 13, 15, 17, 19, 23, 27, 31, 35, 43, 51, 59, 67, 83, 99, 115, 131, 163, 195, 227, 258};
-__constant__ uint8_t LEN_EXTRA[29] = {0, 0, 0, 0, 0, 0, 0, 0, 1, 1, 1, 1, 2, 2, 2, 2, 3, 3, 3, 3, 4, 4, 4, 4, 5, 5, 5, 5, 0};
-__constant__ uint16_t DIST_BASE[30] = {1, 2, 3, 4, 5, 7, 9, 13, 17, 25, 33, 49, 65, 97, 129, 193, 257, 385, 513, 769, 1025, 1537, 2049, 3073, 4097, 6145, 8193, 12289, 16385, 24577};
-__constant__ uint8_t DIST_EXTRA[30] = {0, 0, 0, 0, 1, 1, 2, 2, 3, 3, 4, 4, 5, 5, 6, 6, 7, 7, 8, 8, 9, 9, 10, 10, 11, 11, 12, 12, 13, 13};
-__constant__ uint8_t CL_ORDER[19] = {16, 17, 18, 0, 8, 7, 9, 6, 10, 5, 11, 4, 12, 3, 13, 2, 14, 1, 15};
-
-// status codes per member: 0 ok, >0 error class
-enum { INF_OK = 0, INF_BAD_HEADER = 1, INF_BAD_BLOCK = 2, INF_BAD_CODE = 3, INF_OVERRUN = 4, INF_SIZE = 5 };
-
-__global__ void __launch_bounds__(IW * 32) inflate_warp_kernel(const uint8_t *__restrict__ in, int64_t in_size,
-                                                         const int64_t *__restrict__ cmp_off,
-                                                         const int64_t *__restrict__ ucmp_off, int64_t n_members,
-                                                         uint8_t *__restrict__ out, int64_t out_cap,
-                                                         int32_t *__restrict__ status) {
-    __shared__ WarpTables tabs[IW];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    WarpTables &T = tabs[warp];
-    const int64_t nwarps = (int64_t)gridDim.x * IW;
-    for (int64_t m = (int64_t)blockIdx.x * IW + warp; m < n_members; m += nwarps) {
-        const int64_t c0 = cmp_off[m], c1 = cmp_off[m + 1];
-        const int64_t o0 = ucmp_off[m], o1 = ucmp_off[m + 1];
-        int err = INF_OK;
-        // ---- gzip member header: 10 fixed bytes, FEXTRA (BGZF always), optional name/comment/crc ----
-        int64_t p = c0;
-        if (c1 - c0 < 18 + 8 || c1 > in_size || in[p] != 0x1f || in[p + 1] != 0x8b || in[p + 2] != 8) err = INF_BAD_HEADER;
-        if (!err) {
-            const int flg = in[p + 3];
-            p += 10;
-            if (flg & 4) { const int xlen = in[p] | (in[p + 1] << 8); p += 2 + xlen; }
-            if (flg & 8) { while (p < c1 && in[p]) ++p; ++p; }
-            if (flg & 16) { while (p < c1 && in[p]) ++p; ++p; }
-            if (flg & 2) p += 2;
-            if (p > c1 - 8) err = INF_BAD_HEADER;
-        }
-        BitReader br;
-        br.in = in; br.pos = p; br.end = c1 - 8; br.lim = in_size; br.buf = 0; br.nbits = 0;
-        int64_t opos = o0;
-        bool last = false;
-        while (!err && !last) {
-            // ---- block header (lane 0 reads, everyone follows) -----------------------------------------
-            int btype = 0, hlit = 0, hdist = 0;
-            if (lane == 0) {
-                last = br.get(1) != 0;
-                btype = (int)br.get(2);
-                if (btype == 0) {
-                    br.drop(br.nbits & 7);                       // to a byte boundary
-                    const uint32_t len = br.get(16), nlen = br.get(16);
-                    if ((len ^ 0xffffu) != nlen) err = INF_BAD_BLOCK;
-                    hlit = (int)len;
-                } else if (btype == 2) {
-                    hlit = (int)br.get(5) + 257;
-                    hdist = (int)br.get(5) + 1;
-                    const int hclen = (int)br.get(4) + 4;
-                    if (hlit > 286 || hdist > 30) err = INF_BAD_BLOCK;
-                    // code-length code
-                    uint8_t cl[19];
-                    for (int i = 0; i < 19; ++i) cl[i] = 0;
-                    for (int i = 0; i < hclen; ++i) cl[CL_ORDER[i]] = (uint8_t)br.get(3);
-                    // tiny canonical decoder for the 19-symbol code, bit by bit
-                    uint16_t ccnt[8], csym[19];
-                    for (int i = 0; i < 8; ++i) ccnt[i] = 0;
-                    for (int i = 0; i < 19; ++i) ccnt[cl[i]]++;
-                    int offs[8];
-                    offs[1] = 0;
-                    for (int i = 1; i < 7; ++i) offs[i + 1] = offs[i] + ccnt[i];
-                    for (int i = 0; i < 19; ++i)
-                        if (cl[i]) csym[offs[cl[i]]++] = (uint16_t)i;
-                    int idx = 0;
-                    while (!err && idx < hlit + hdist) {
-                        int code = 0, first = 0, index = 0, sym = -1;
-                        for (int len = 1; len <= 7; ++len) {
-                            code |= (int)br.get(1);
-                            const int count = ccnt[len];
-                            if (code - count < first) { sym = csym[index + (code - first)]; break; }
-                            index += count; first += count; first <<= 1; code <<= 1;
-                        }
-                        if (sym < 0) { err = INF_BAD_CODE; break; }
-                        if (sym < 16) T.lens[idx++] = (uint8_t)sym;
-                        else {
-                            int rep, val = 0;
-                            if (sym == 16) { if (idx == 0) { err = INF_BAD_CODE; break; } val = T.lens[idx - 1]; rep = 3 + (int)br.get(2); }
-                            else if (sym == 17) rep = 3 + (int)br.get(3);
-                            else rep = 11 + (int)br.get(7);
-                            if (idx + rep > hlit + hdist) { err = INF_BAD_CODE; break; }
-                            while (rep--) T.lens[idx++] = (uint8_t)val;
-                        }
-                    }
-                    if (!err && T.lens[256] == 0) err = INF_BAD_CODE;
-                } else if (btype == 3) err = INF_BAD_BLOCK;
-                if (br.overrun()) err = INF_OVERRUN;
-            }
-            err = __shfl_sync(0xffffffffu, err, 0);
-            btype = __shfl_sync(0xffffffffu, btype, 0);
-            hlit = __shfl_sync(0xffffffffu, hlit, 0);
-            hdist = __shfl_sync(0xffffffffu, hdist, 0);
-            last = __shfl_sync(0xffffffffu, (int)last, 0) != 0;
-            if (err) break;
-            if (btype == 0) {
-                // ---- stored block: warp-wide byte copy ------------------------------------------------------
-                int64_t src = 0;
-                if (lane == 0) { src = br.pos - (br.nbits >> 3); }
-                src = shfl_i64(src, 0);
-                const int len = hlit;
-                if (src + len > c1 - 8 || opos + len > o1 || opos + len > out_cap) { err = INF_OVERRUN; break; }
-                for (int i = lane; i < len; i += 32) out[opos + i] = in[src + i];
-                opos += len;
-                if (lane == 0) { br.pos = src + len; br.buf = 0; br.nbits = 0; }
-                __syncwarp();
-                continue;
-            }
-            // ---- Huffman tables (fixed or dynamic) ---------------------------------------------------------
-            if (btype == 1) {
-                for (int i = lane; i < 288; i += 32) T.lens[i] = (uint8_t)(i < 144 ? 8 : (i < 256 ? 9 : (i < 280 ? 7 : 8)));
-                for (int i = lane; i < 30; i += 32) T.lens[288 + i] = 5;
-                hlit = 288; hdist = 30;
-            }
-            __syncwarp();
-            bool ok = build_table(T.lens, hlit, T.lit, LIT_BITS, 9, T.litcnt, T.litsym, lane);
-            ok = build_table(T.lens + hlit, hdist, T.dist, DIST_BITS, 5, T.distcnt, T.distsym, lane) && ok;
-            // an incomplete distance code with a single symbol is legal; over-subscription is not
-            if (!ok) { err = INF_BAD_CODE; break; }
-            // second literal: where the bits left over after a literal decode another literal completely, one
-            // table lookup yields both (DNA text: ~2-bit codes, so most lookups)
-            for (int i = lane; i < (1 << LIT_BITS); i += 32) {
-                const uint32_t e1 = T.lit[i] & 0xffffu;
-                const uint32_t l1 = e1 >> 9;
-                if (e1 && (e1 & 511u) < 256u) {
-                    const uint32_t e2 = T.lit[i >> l1] & 0xffffu;       // low halves never change in this pass
-                    const uint32_t l2 = e2 >> 9;
-                    if (e2 && (e2 & 511u) < 256u && l1 + l2 <= (uint32_t)LIT_BITS)
-                        T.lit[i] = e1 | TWO_LIT | ((l1 + l2) << 24) | ((e2 & 255u) << 16);
-                }
-            }
-            __syncwarp();
-            // ---- symbol loop: lane 0 decodes literals until a match / end of block, matches are copied by
-            //      the whole warp ---------------------------------------------------------------------------------
-            bool eob = false;
-            while (!eob && !err) {
-                int mlen = 0, mdist = 0;
-                if (lane == 0) {
-                    while (true) {
-                        // fast path: one or two literals per table lookup
-                        {
-                            uint64_t buf = br.buf;
-                            int nbits = br.nbits;
-                            int64_t pos = br.pos;
-                            const int64_t olim = (o1 < out_cap ? o1 : out_cap) - 2;
-                            while (opos <= olim) {
-                                if (nbits < 32) {
-                                    if (pos + 8 > br.lim) break;
-                                    const uint32_t *w = reinterpret_cast<const uint32_t *>(in + (pos & ~(int64_t)3));
-                                    const uint32_t v = __funnelshift_r(__ldg(w), __ldg(w + 1), (int)(pos & 3) * 8);
-                                    buf |= (uint64_t)v << nbits;
-                                    nbits += 32;
-                                    pos += 4;
-                                }
-                                const uint32_t e = T.lit[(uint32_t)buf & ((1u << LIT_BITS) - 1u)];
-                                if (e & TWO_LIT) {
-                                    out[opos] = (uint8_t)e;
-                                    out[opos + 1] = (uint8_t)(e >> 16);
-                                    opos += 2;
-                                    const int l = (int)((e >> 24) & 15u);
-                                    buf >>= l; nbits -= l;
-                                } else if ((e & 0xffffu) != 0u && (e & 511u) < 256u) {
-                                    out[opos++] = (uint8_t)e;
-                                    const int l = (int)((e >> 9) & 15u);
-                                    buf >>= l; nbits -= l;
-                                } else break;
-                            }
-                            br.buf = buf; br.nbits = nbits; br.pos = pos;
-                        }
-                        br.refill32();
-                        int sym;
-                        const uint32_t e = T.lit[br.peek(LIT_BITS)] & 0xffffu;
-                        if (e) { br.drop(e >> 9); sym = e & 511; }
-                        else sym = slow_decode(br, T.litcnt, T.litsym);
-                        if (sym < 0) { err = INF_BAD_CODE; break; }
-                        if (sym < 256) {
-                            if (opos >= o1 || opos >= out_cap) { err = INF_OVERRUN; break; }
-                            out[opos++] = (uint8_t)sym;
-                            continue;
-                        }
-                        if (sym == 256) { eob = true; break; }
-                        sym -= 257;
-                        if (sym >= 29) { err = INF_BAD_CODE; break; }
-                        br.refill32();
-                        mlen = LEN_BASE[sym] + (int)br.peek(LEN_EXTRA[sym]);
-                        br.drop(LEN_EXTRA[sym]);
-                        br.refill32();
-                        int ds;
-                        const uint16_t de = T.dist[br.peek(DIST_BITS)];
-                        if (de) { br.drop(de >> 5); ds = de & 31; }
-                        else ds = slow_decode(br, T.distcnt, T.distsym);
-                        if (ds < 0 || ds >= 30) { err = INF_BAD_CODE; break; }
-                        br.refill32();
-                        mdist = DIST_BASE[ds] + (int)br.peek(DIST_EXTRA[ds]);
-                        br.drop(DIST_EXTRA[ds]);
-                        if (mdist > opos - o0) { err = INF_BAD_CODE; break; }        // BGZF members are self-contained
-                        if (opos + mlen > o1 || opos + mlen > out_cap) { err = INF_OVERRUN; break; }
-                        if (mlen <= SHORT_MATCH) {                                       // short match: copied right here
-                            const int64_t src = opos - mdist;
-                            if (mdist >= mlen && (src & ~(int64_t)7) + 32 <= out_cap) {
-                                // no overlap: fetch the whole source with four aligned 8-byte loads issued together
-                                // (ONE L2 round trip per match instead of one per byte), then store from registers
-                                const uint64_t *w = reinterpret_cast<const uint64_t *>(out + (src & ~(int64_t)7));
-                                const uint64_t a0 = w[0], a1 = w[1], a2 = w[2], a3 = w[3];
-                                const int sh = (int)(src & 7) * 8;
-                                uint64_t v0 = a0, v1 = a1, v2 = a2;
-                                if (sh) {
-                                    v0 = (a0 >> sh) | (a1 << (64 - sh));
-                                    v1 = (a1 >> sh) | (a2 << (64 - sh));
-                                    v2 = (a2 >> sh) | (a3 << (64 - sh));
-                                }
-                                uint8_t *o = out + opos;
-#pragma unroll
-                                for (int i = 0; i < 8; ++i) if (i < mlen) o[i] = (uint8_t)(v0 >> (8 * i));
-                                if (mlen > 8) {
-#pragma unroll
-                                    for (int i = 0; i < 8; ++i) if (8 + i < mlen) o[8 + i] = (uint8_t)(v1 >> (8 * i));
-                                    if (mlen > 16) {
-#pragma unroll
-                                        for (int i = 0; i < 8; ++i) if (16 + i < mlen) o[16 + i] = (uint8_t)(v2 >> (8 * i));
-                                    }
-                                }
-                            } else {
-                                for (int i = 0; i < mlen; ++i) out[opos + i] = out[src + i];   // in order: overlap repeats
-                            }
-                            opos += mlen;
-                            mlen = 0;
-                            continue;
-                        }
-                        break;
-                    }
-                    if (br.overrun()) err = INF_OVERRUN;
-                }
-                __syncwarp();
-                err = __shfl_sync(0xffffffffu, err, 0);
-                eob = __shfl_sync(0xffffffffu, (int)eob, 0) != 0;
-                mlen = __shfl_sync(0xffffffffu, mlen, 0);
-                mdist = __shfl_sync(0xffffffffu, mdist, 0);
-                opos = shfl_i64(opos, 0);
-                if (err || eob) break;
-                if (mlen > 0) {
-                    __threadfence_block();
-                    const int64_t src = opos - mdist;
-                    for (int i = lane; i < mlen; i += 32) out[opos + i] = out[src + (mdist >= mlen ? i : i % mdist)];
-                    opos += mlen;
-                    __syncwarp();
-                }
-            }
-        }
-        if (!err && opos != o1) err = INF_SIZE;
-        if (lane == 0) status[m] = err;
-        __syncwarp();
-    }
-}
-
 // ---- a thread per member -----------------------------------------------------------------------------
-// The Huffman decode of one member is serial, so the warp-per-member kernel above issues every instruction
-// for ONE useful lane.  Here 32 members share a warp: each lane runs fxi::inflate_member on its own member
+// The Huffman decode of one member is serial: a warp working on one member would issue every instruction
+// for ONE useful lane.  Here 32 members share a warp: each lane runs an fxi::Decoder on its own member
 // with its own 2.2 KB of decode tables; up to 1,152 members are in flight per SM.
 __device__ const uint16_t D_LEN_BASE[29] = {3, 4, 5, 6, 7, 8, 9, 10, 11, 13, 15, 17, 19, 23, 27, 31, 35, 43, 51, 59, 67, 83, 99, 115, 131, 163, 195, 227, 258};
 __device__ const uint8_t D_LEN_EXTRA[29] = {0, 0, 0, 0, 0, 0, 0, 0, 1, 1, 1, 1, 2, 2, 2, 2, 3, 3, 3, 3, 4, 4, 4, 4, 5, 5, 5, 5, 0};
@@ -461,10 +81,9 @@ __global__ void __launch_bounds__(MT_THREADS, MT_WARPS_PER_SM * 32 / MT_THREADS)
 // One thread per member, slicing-by-4 with the four 256-entry tables in shared memory; 16-byte loads once the output
 // pointer is aligned.  Sets status 9 for a member whose inflate status was 0 and whose CRC differs.
 constexpr int CRC_THREADS = 128;
-__global__ void __launch_bounds__(CRC_THREADS) crc_members_kernel(const uint8_t *__restrict__ comp, const int64_t *__restrict__ cmp_off,
-                                                                  const int64_t *__restrict__ ucmp_off, int64_t n_members,
-                                                                  const uint8_t *__restrict__ out, int32_t *__restrict__ status) {
-    __shared__ uint32_t T[4][256];
+
+// The four slicing-by-4 tables of CRC-32 (polynomial 0xEDB88320), built by the whole CTA into shared memory.
+__device__ __forceinline__ void crc_build_tables(uint32_t (*T)[256]) {
     for (int i = threadIdx.x; i < 256; i += CRC_THREADS) {
         uint32_t c = (uint32_t)i;
         for (int k = 0; k < 8; ++k) c = (c >> 1) ^ (0xEDB88320u & (0u - (c & 1u)));
@@ -476,10 +95,10 @@ __global__ void __launch_bounds__(CRC_THREADS) crc_members_kernel(const uint8_t 
         for (int t = 1; t < 4; ++t) { c = T[0][c & 0xffu] ^ (c >> 8); T[t][i] = c; }
     }
     __syncthreads();
-    const int64_t m = (int64_t)blockIdx.x * CRC_THREADS + threadIdx.x;
-    if (m >= n_members || status[m] != 0) return;
-    const uint8_t *p = out + ucmp_off[m];
-    int64_t len = ucmp_off[m + 1] - ucmp_off[m];
+}
+
+// CRC-32 of p[0, len): bytewise up to 16-byte alignment, then four words per 16-byte load, then the tail bytewise.
+__device__ __forceinline__ uint32_t crc32_range(const uint32_t (*T)[256], const uint8_t *p, int64_t len) {
     uint32_t crc = 0xffffffffu;
     auto word = [&](uint32_t w) {
         crc ^= w;
@@ -491,7 +110,17 @@ __global__ void __launch_bounds__(CRC_THREADS) crc_members_kernel(const uint8_t 
         word(v.x); word(v.y); word(v.z); word(v.w);
     }
     for (; len > 0; --len, ++p) crc = T[0][(crc ^ *p) & 0xffu] ^ (crc >> 8);
-    crc = ~crc;
+    return ~crc;
+}
+
+__global__ void __launch_bounds__(CRC_THREADS) crc_members_kernel(const uint8_t *__restrict__ comp, const int64_t *__restrict__ cmp_off,
+                                                                  const int64_t *__restrict__ ucmp_off, int64_t n_members,
+                                                                  const uint8_t *__restrict__ out, int32_t *__restrict__ status) {
+    __shared__ uint32_t T[4][256];
+    crc_build_tables(T);
+    const int64_t m = (int64_t)blockIdx.x * CRC_THREADS + threadIdx.x;
+    if (m >= n_members || status[m] != 0) return;
+    const uint32_t crc = crc32_range(T, out + ucmp_off[m], ucmp_off[m + 1] - ucmp_off[m]);
     const uint8_t *t = comp + cmp_off[m + 1] - 8;                      // CRC32, ISIZE: the last eight bytes of the member
     const uint32_t want = (uint32_t)t[0] | ((uint32_t)t[1] << 8) | ((uint32_t)t[2] << 16) | ((uint32_t)t[3] << 24);
     if (crc != want) status[m] = 9;
@@ -517,37 +146,14 @@ __global__ void __launch_bounds__(64) inflate_points_kernel(const uint8_t *__res
                                      wi >= 0 ? windows + (size_t)wi * wsize : nullptr, wi >= 0 ? wsize : 0, tables[i], K);
 }
 
-// CRC-32 of out[off[i], off[i + 1]) per segment (slicing-by-4, as crc_members_kernel)
+// CRC-32 of out[off[i], off[i + 1]) per segment
 __global__ void __launch_bounds__(CRC_THREADS) crc_segments_kernel(const int64_t *__restrict__ off, int64_t n, const uint8_t *__restrict__ out,
                                                                    uint32_t *__restrict__ crc_out) {
     __shared__ uint32_t T[4][256];
-    for (int i = threadIdx.x; i < 256; i += CRC_THREADS) {
-        uint32_t c = (uint32_t)i;
-        for (int k = 0; k < 8; ++k) c = (c >> 1) ^ (0xEDB88320u & (0u - (c & 1u)));
-        T[0][i] = c;
-    }
-    __syncthreads();
-    for (int i = threadIdx.x; i < 256; i += CRC_THREADS) {
-        uint32_t c = T[0][i];
-        for (int t = 1; t < 4; ++t) { c = T[0][c & 0xffu] ^ (c >> 8); T[t][i] = c; }
-    }
-    __syncthreads();
+    crc_build_tables(T);
     const int64_t m = (int64_t)blockIdx.x * CRC_THREADS + threadIdx.x;
     if (m >= n) return;
-    const uint8_t *p = out + off[m];
-    int64_t len = off[m + 1] - off[m];
-    uint32_t crc = 0xffffffffu;
-    auto word = [&](uint32_t w) {
-        crc ^= w;
-        crc = T[3][crc & 0xffu] ^ T[2][(crc >> 8) & 0xffu] ^ T[1][(crc >> 16) & 0xffu] ^ T[0][crc >> 24];
-    };
-    while (len > 0 && (reinterpret_cast<uintptr_t>(p) & 15u)) { crc = T[0][(crc ^ *p) & 0xffu] ^ (crc >> 8); ++p; --len; }
-    for (; len >= 16; len -= 16, p += 16) {
-        const uint4 v = *reinterpret_cast<const uint4 *>(p);
-        word(v.x); word(v.y); word(v.z); word(v.w);
-    }
-    for (; len > 0; --len, ++p) crc = T[0][(crc ^ *p) & 0xffu] ^ (crc >> 8);
-    crc_out[m] = ~crc;
+    crc_out[m] = crc32_range(T, out + off[m], off[m + 1] - off[m]);
 }
 
 }  // namespace fxg
@@ -607,22 +213,14 @@ extern "C" int fxg_inflate_members_dev(fxg_ctx *ctx, const fxg_file *compressed,
     FXG_CHECK_ARG(d_cmp_off && d_ucmp_off && d_out && d_status, "null device pointer");
     FXG_CUDA(cudaSetDevice(ctx->device));
     FxgProfScope prof(ctx, FXG_PROF_GATHER);
-    if (getenv("FXG_INFLATE_WARP_PER_MEMBER")) {                 // A/B and debugging
-        int64_t blocks = (n_members + IW - 1) / IW;
-        const int64_t maxb = (int64_t)ctx->sm_count * 6;
-        if (blocks > maxb) blocks = maxb;
-        inflate_warp_kernel<<<(unsigned)blocks, IW * 32, 0, ctx->stream>>>(compressed->d, compressed->size, d_cmp_off, d_ucmp_off,
-                                                                           n_members, d_out, out_cap, d_status);
-    } else {
-        int64_t blocks = (n_members + MT_THREADS - 1) / MT_THREADS;
-        const int64_t maxb = (int64_t)ctx->sm_count * (MT_WARPS_PER_SM * 32 / MT_THREADS);
-        if (blocks > maxb) blocks = maxb;
-        int rc = ctx->misc.reserve((size_t)blocks * MT_THREADS * sizeof(fxi::MemberTables));
-        if (rc) return rc;
-        inflate_thread_kernel<<<(unsigned)blocks, MT_THREADS, 0, ctx->stream>>>(compressed->d, compressed->size, d_cmp_off, d_ucmp_off,
-                                                                                n_members, d_out, out_cap, d_status,
-                                                                                (fxi::MemberTables *)ctx->misc.ptr);
-    }
+    int64_t blocks = (n_members + MT_THREADS - 1) / MT_THREADS;
+    const int64_t maxb = (int64_t)ctx->sm_count * (MT_WARPS_PER_SM * 32 / MT_THREADS);
+    if (blocks > maxb) blocks = maxb;
+    int rc = ctx->misc.reserve((size_t)blocks * MT_THREADS * sizeof(fxi::MemberTables));
+    if (rc) return rc;
+    inflate_thread_kernel<<<(unsigned)blocks, MT_THREADS, 0, ctx->stream>>>(compressed->d, compressed->size, d_cmp_off, d_ucmp_off,
+                                                                            n_members, d_out, out_cap, d_status,
+                                                                            (fxi::MemberTables *)ctx->misc.ptr);
     FXG_CUDA(cudaGetLastError());
     const char *ce = getenv("FXG_BGZF_CRC");
     if (!(ce && ce[0] == '0')) {                                 // member CRCs against their trailers (status 9 = mismatch)

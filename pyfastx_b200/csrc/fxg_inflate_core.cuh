@@ -1,6 +1,6 @@
 // fxg_inflate_core.cuh -- one DEFLATE (RFC 1951) member decoded by ONE thread.
 //
-// Used by inflate_kernel (fxg_inflate.cu) with a thread per BGZF member: 32 members per warp, so the
+// Used by inflate_thread_kernel (fxg_inflate.cu) with a thread per BGZF member: 32 members per warp, so the
 // serial Huffman decode -- which cannot be spread over the lanes of a warp -- still fills every lane.
 // The code is plain C++ (no CUDA intrinsics) so that tests/test_inflate_core_cpu.py can compile the very
 // same functions for the host and check them against zlib without a GPU.  Nothing here is a CPU fallback:

@@ -13,17 +13,21 @@
 //           {#newlines, #header starts}.  This kernel carries all of the file traffic and is
 //           a pure stream: nothing in it waits on another CTA.
 //   prefix  exclusive prefix of the region counts (three small kernels over 4 bytes per region).
-//   lines   one thread per LINE, reading only the newline list.  Every quantity the reference
-//           carries from line to line is re-expressed as a local rule on (this line, previous
-//           line, global line index, global header ordinal):
+//   rows    reads only the newline list (and the file bytes of header / read-name lines).  Every
+//           quantity the reference carries from line to line is re-expressed as a local rule on
+//           (this line, previous line, global line index, global header ordinal):
 //             - a header line writes boff / dlen / elen / name length / its line index;
 //             - a sequence line that follows a header writes llen;
 //             - a sequence line whose length differs from the previous sequence line raises an
-//               "event" (count, min/max line index, sum of length deltas) on its record;
-//           a tiny finalize kernel then derives blen, slen, norm per record from neighbouring
-//           headers and the event summary (proof of equivalence with index.c:325-342 in DESIGN.md).
-//           FASTQ needs no per-record state at all: line k of the file writes field k%4 of row k/4.
-//           File bytes are touched again only for header / read-name lines (the name cut).
+//               "event" (count, min/max line index, sum of length deltas) on its record.
+//           FASTA (fasta_lines_kernel): one lane per region walks only the lines that matter, found
+//           from the records mark left behind; a tiny finalize kernel then derives blen, slen, norm
+//           per record from neighbouring headers and the event summary (proof of equivalence with
+//           index.c:325-342 in DESIGN.md).
+//           FASTQ (fastq_records_kernel): no per-record state at all, line k of the file writes
+//           field k%4 of row k/4; one lane builds the whole row of a read from five consecutive
+//           newline positions, and reads the name line once to find the name cut.
+//           Regions the fast paths cannot settle go through full_region, lane per line.
 //
 // An earlier single-pass variant (TMA tile ring + decoupled look-back inside one kernel) stayed far below
 // DRAM speed: every tile's shared-memory slot stayed occupied for the thousands of cycles its look-back spent
@@ -40,7 +44,7 @@ namespace fxg {
 #endif
 constexpr int REGION   = 2048;            // bytes per warp
 constexpr int SEGCAP   = 128;             // newline-list entries kept per region (lines >= 16 B on average)
-constexpr int MARK_WARPS = 8;             // warps per CTA of the mark / lines kernels
+constexpr int MARK_WARPS = 8;             // warps per CTA of the mark / rows kernels
 constexpr int PS_THREADS = 256, PS_PER_THREAD = 16, PS_BLOCK = PS_THREADS * PS_PER_THREAD;   // regions per prefix block
 constexpr int64_t NOPOS = INT64_MIN / 4;
 constexpr uint32_t E_POS = 0x07ffu, E_CR = 1u << 14, E_HDR = 1u << 15;
@@ -88,8 +92,6 @@ struct ScanParams {
                             // (padded to PS_BLOCK with zeros)
     uint4    *rec2;         // FASTA, per region: {first entry | second << 16, interesting-line mask, header mask, 0}
     uint16_t *seg;          // per region: SEGCAP entries, file order
-    uint8_t  *cut;          // FASTQ, per entry: name cut of the line FOLLOWING that newline if it starts with '@'
-                            // (offset of the first ' ' after the '@'; 254 = no blank in the line; 255 = not examined)
     ulonglong2 *ex;         // per region: exclusive {newlines, header starts}
     ulonglong2 *bs;         // per prefix block
     ScanTotals *totals;
@@ -109,67 +111,19 @@ __device__ __forceinline__ uint4 ld_stream16(const uint8_t *p) {
     return v;
 }
 
-// FASTQ name cut (fastq.c:104-117: the name ends at the first ' ', strchr semantics) of a line that begins
-// with '@' at region byte a-1, found by mark while the bytes are on chip: the rows kernel otherwise has to fetch the
-// start of every name line from DRAM a second time just to find the first blank -- several times the 32-byte row in
-// DRAM reads per read.
-// Loop-free probe of the FXG_CUT_WORDS aligned words that follow the '@' in the region's shared-memory copy: a SWAR
-// "byte < 0x21" test per word, the per-byte flags packed four to a nibble by one multiply (on the FMA pipe) so that
-// the position of the first such byte is one find-first-set.  The first byte below 0x21 decides -- ' ' -> its offset;
-// '\n', NUL or "\r\n" -> 254 (no blank: the whole line); anything else (tab, lone '\r'), a window without such a
-// byte or one that runs past the region -> 255 = the rows kernel searches the file for that read.
-#ifndef FXG_MARK_CUT
-#define FXG_MARK_CUT 0
-#endif
-#ifndef FXG_CUT_WORDS
-#define FXG_CUT_WORDS 6
-#endif
-__device__ __forceinline__ uint32_t swz_unit(uint32_t u);
-template <int V> __device__ __forceinline__ uint32_t region_byte(const uint8_t *sb, uint32_t p);
-template <int V>
-__device__ __forceinline__ uint32_t name_cut_smem(const uint8_t *sb, uint32_t a) {
-    uint32_t M = 0;                                                               // bit p <-> byte 4 * (a >> 2) + p
-#pragma unroll
-    for (int k = 0; k < FXG_CUT_WORDS; ++k) {
-        const uint32_t wq = min((a >> 2) + (uint32_t)k, (uint32_t)(REGION / 4 - 1));   // stays inside the region's copy
-        const uint32_t w = reinterpret_cast<const uint32_t *>(sb)[V == 2 ? ((swz_unit(wq >> 2) << 2) | (wq & 3u)) : wq];
-        const uint32_t lt = ~((((w & 0x7f7f7f7fu) + 0x5f5f5f5fu) | w)) & 0x80808080u;      // 0x80 per byte below 0x21
-        M |= ((lt * 0x00204081u) >> 28) << (4 * k);
-    }
-    M &= 0xffffffffu << (a & 3u);                                                 // bytes before the name
-    if (!M) return 255u;
-    const uint32_t p = (a & ~3u) + (uint32_t)(__ffs(M) - 1);
-    if (p >= (uint32_t)REGION) return 255u;
-    if (p >= ((a >> 2) + (uint32_t)FXG_CUT_WORDS) * 4u) return 255u;               // (clamped word read twice)
-    const uint32_t b = region_byte<V>(sb, p);
-    if (b == ' ') return p - a;                                                   // < 4 * FXG_CUT_WORDS <= 32
-    if (b == '\n' || b == 0u) return 254u;
-    if (b == '\r' && p + 1u < (uint32_t)REGION && region_byte<V>(sb, p + 1u) == '\n') return 254u;
-    return 255u;
-}
-
 // =============================================================================================
 // mark: newline list + counts of one 2 KiB region per warp
 // =============================================================================================
-// FXG_MARK_V = 2 (r02): every lane tests 64 CONTIGUOUS bytes.  The loads stay coalesced (lane l takes 16 bytes of each
+// Pass 1, V = 2 (r02): every lane tests 64 CONTIGUOUS bytes.  The loads stay coalesced (lane l takes 16 bytes of each
 // of the four 512-byte quarters); the region is transposed on its way through shared memory, where pass 2 needs it
 // anyway: 16-byte unit u is stored at u ^ ((u >> 3) & 7), which makes both the quarter-major stores and the lane-major
 // loads (units 4l .. 4l+3) bank-conflict free.  With contiguous bytes per lane the file order of the newlines is the
 // lane order, so ONE pair of ballots ranks the whole region (r01: one or two ballots and a rank per quarter), and
 // the per-byte flags are packed into a position-ordered 64-bit mask by integer multiply-adds -- work for the FMA pipe
-// where the r01 code kept the ALU pipe busy.
-// Which pass 1 a mode uses is a compile-time choice: see DESIGN.md section 3.
-#ifndef FXG_MARK_V_FASTA
-#define FXG_MARK_V_FASTA 1
-#endif
-#ifndef FXG_MARK_V_FASTQ
-#define FXG_MARK_V_FASTQ 2
-#endif
-#ifndef FXG_MARK_RPW
-#define FXG_MARK_RPW 1            // consecutive regions per warp.  > 1: the loads of region i + 1 are in flight while region i is
-                                  // worked on -- measured slower (2, 4, 8 regions at 4 or 5 CTAs per SM for the extra registers) than
-                                  // one region per warp at 6 CTAs per SM; the kernel is bound by instruction issue, not by latency
-#endif
+// where the r01 code kept the ALU pipe busy.  V = 1 tests every 16-byte chunk where it was loaded.
+// One region per warp: a warp that also had the next region's loads in flight was slower (2, 4, 8 regions at 4 or 5
+// CTAs per SM for the extra registers) than one region per warp at 6 CTAs per SM; the kernel is bound by instruction
+// issue, not by latency.
 __device__ __forceinline__ uint32_t swz_unit(uint32_t u) { return u ^ ((u >> 3) & 7u); }
 // byte p (0 .. REGION-1) of a region held in swizzled (V = 2) or linear (V = 1) shared memory
 template <int V>
@@ -179,182 +133,172 @@ __device__ __forceinline__ uint32_t region_byte(const uint8_t *sb, uint32_t p) {
 
 template <int MODE, int V>   // MODE: 0 = FASTA, 1 = FASTQ; V: pass-1 variant
 __global__ void __launch_bounds__(MARK_WARPS * 32, FXG_MARK_MINB) mark_kernel(const ScanParams P) {
-    __shared__ uint4    s_data[MARK_WARPS * (REGION / 16) + (FXG_MARK_CUT ? 2 : 0)];   // the regions' bytes (neighbour-byte lookups; + 32 B: the name probe of the last warp may read past its region)
+    __shared__ uint4    s_data[MARK_WARPS * (REGION / 16)];   // the regions' bytes (neighbour-byte lookups)
     __shared__ uint16_t s_ent[MARK_WARPS][SEGCAP];         // newline positions, then complete entries
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int64_t r0 = ((int64_t)blockIdx.x * MARK_WARPS + warp) * FXG_MARK_RPW;
-    if (r0 >= P.nreg) return;
+    const int64_t r = (int64_t)blockIdx.x * MARK_WARPS + warp;
+    if (r >= P.nreg) return;
     const uint32_t lt_mask = (1u << lane) - 1u;
     const int64_t n = P.n;
     const uint8_t *file = P.file;
     const uint32_t k0a = reg_const(0x0a0a0a0au), k7f = reg_const(0x7f7f7f7fu), k80 = reg_const(0x80808080u);
-
-    // the 2 KiB of region rr: four coalesced 16-byte streaming loads per lane, all in flight together
-    auto load_region = [&](int64_t rr, uint4 (&vv)[4]) {
-        const int64_t base = rr * REGION;
-        if (base + REGION <= n) {
-            const uint8_t *src = file + base + lane * 16;
-#pragma unroll
-            for (int j = 0; j < 4; ++j) vv[j] = ld_stream16(src + j * 512);
-        } else {
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                const int64_t o = base + j * 512 + lane * 16;
-                if (o + 16 <= n) { vv[j] = ld_stream16(file + o); continue; }
-                // the chunk that contains EOF (or lies past it): bytes >= n read as 0, and a file that does
-                // not end in '\n' gets a virtual newline at n (kseq returns the last line all the same)
-                const bool virt = n > 0 && file[n - 1] != '\n';
-                uint32_t w[4] = {0, 0, 0, 0};
-                for (int i = 0; i < 16; ++i) {
-                    const int64_t x = o + i;
-                    const uint32_t b = x < n ? file[x] : ((virt && x == n) ? 0x0au : 0u);
-                    w[i >> 2] |= b << ((i & 3) * 8);
-                }
-                vv[j] = make_uint4(w[0], w[1], w[2], w[3]);
-            }
-        }
-    };
-    uint4 vn[4];
-    load_region(r0, vn);
-#pragma unroll 1
-    for (int it = 0; it < FXG_MARK_RPW; ++it) {
-    const int64_t r = r0 + it;
-    if (r >= P.nreg) break;
     const int64_t base = r * REGION;
-    uint4 v[4] = {vn[0], vn[1], vn[2], vn[3]};
-    if (it + 1 < FXG_MARK_RPW && r + 1 < P.nreg) load_region(r + 1, vn);     // prefetch: in flight during this region's work
+
+    // the 2 KiB of the region: four coalesced 16-byte streaming loads per lane, all in flight together
+    uint4 v[4];
+    if (base + REGION <= n) {
+        const uint8_t *src = file + base + lane * 16;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) v[j] = ld_stream16(src + j * 512);
+    } else {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int64_t o = base + j * 512 + lane * 16;
+            if (o + 16 <= n) { v[j] = ld_stream16(file + o); continue; }
+            // the chunk that contains EOF (or lies past it): bytes >= n read as 0, and a file that does
+            // not end in '\n' gets a virtual newline at n (kseq returns the last line all the same)
+            const bool virt = n > 0 && file[n - 1] != '\n';
+            uint32_t w[4] = {0, 0, 0, 0};
+            for (int i = 0; i < 16; ++i) {
+                const int64_t x = o + i;
+                const uint32_t b = x < n ? file[x] : ((virt && x == n) ? 0x0au : 0u);
+                w[i >> 2] |= b << ((i & 3) * 8);
+            }
+            v[j] = make_uint4(w[0], w[1], w[2], w[3]);
+        }
+    }
     uint32_t nlc = 0;
     uint16_t *ent = s_ent[warp];
 
     if constexpr (V == 2) {
-    // ---- pass 1 (V2): transpose through shared memory, 64 contiguous bytes per lane, one ranking for the region ----
-    uint4 *sd = s_data + warp * (REGION / 16);
+        // ---- pass 1 (V2): transpose through shared memory, 64 contiguous bytes per lane, one ranking for the region ----
+        uint4 *sd = s_data + warp * (REGION / 16);
 #pragma unroll
-    for (int j = 0; j < 4; ++j) sd[swz_unit((uint32_t)(j * 32 + lane))] = v[j];
-    __syncwarp();
-    uint32_t lo = 0, hi = 0;                      // bit p of hi:lo <-> byte 64 * lane + p is a newline
+        for (int j = 0; j < 4; ++j) sd[swz_unit((uint32_t)(j * 32 + lane))] = v[j];
+        __syncwarp();
+        uint32_t lo = 0, hi = 0;                      // bit p of hi:lo <-> byte 64 * lane + p is a newline
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        const uint4 x = sd[swz_unit((uint32_t)(4 * lane + i))];
-        const uint32_t w4[4] = {x.x, x.y, x.z, x.w};
+        for (int i = 0; i < 4; ++i) {
+            const uint4 x = sd[swz_unit((uint32_t)(4 * lane + i))];
+            const uint32_t w4[4] = {x.x, x.y, x.z, x.w};
 #pragma unroll
-        for (int c = 0; c < 4; ++c) {
-            const uint32_t f = byte_eq_mask_r(w4[c], k0a, k7f, k80);            // 0x80 per newline byte
-            const uint32_t nib = (f * 0x00204081u) >> 28;                       // the four flags as a nibble, byte order
-            const int k = 4 * i + c;
-            if (k < 8) lo = nib * (1u << (4 * k)) + lo;                         // multiply-adds: FMA pipe
-            else hi = nib * (1u << (4 * (k - 8))) + hi;
+            for (int c = 0; c < 4; ++c) {
+                const uint32_t f = byte_eq_mask_r(w4[c], k0a, k7f, k80);            // 0x80 per newline byte
+                const uint32_t nib = (f * 0x00204081u) >> 28;                       // the four flags as a nibble, byte order
+                const int k = 4 * i + c;
+                if (k < 8) lo = nib * (1u << (4 * k)) + lo;                         // multiply-adds: FMA pipe
+                else hi = nib * (1u << (4 * (k - 8))) + hi;
+            }
         }
-    }
-    {
-        const uint32_t c = (uint32_t)(__popc(lo) + __popc(hi));
-        const uint32_t b1 = __ballot_sync(0xffffffffu, c >= 1u), b2 = __ballot_sync(0xffffffffu, c >= 2u);
-        const uint32_t b3 = __ballot_sync(0xffffffffu, c >= 3u);
-        const uint32_t pbase = (uint32_t)lane * 64u;
-        if (!b3) {
-            // lines of 32 bytes or more: at most two newlines in a lane's 64 bytes
-            const uint32_t idx = (uint32_t)(__popc(b1 & lt_mask) + __popc(b2 & lt_mask));
-            nlc = (uint32_t)(__popc(b1) + __popc(b2));
-            if (c) {
-                const uint32_t p1 = lo ? (uint32_t)(__ffs(lo) - 1) : 32u + (uint32_t)(__ffs(hi) - 1);
-                if (idx < (uint32_t)SEGCAP) ent[idx] = (uint16_t)(pbase + p1);
-                if (c >= 2u) {
-                    if (lo) lo &= lo - 1u; else hi &= hi - 1u;
-                    const uint32_t p2 = lo ? (uint32_t)(__ffs(lo) - 1) : 32u + (uint32_t)(__ffs(hi) - 1);
-                    if (idx + 1u < (uint32_t)SEGCAP) ent[idx + 1u] = (uint16_t)(pbase + p2);
+        {
+            const uint32_t c = (uint32_t)(__popc(lo) + __popc(hi));
+            const uint32_t b1 = __ballot_sync(0xffffffffu, c >= 1u), b2 = __ballot_sync(0xffffffffu, c >= 2u);
+            const uint32_t b3 = __ballot_sync(0xffffffffu, c >= 3u);
+            const uint32_t pbase = (uint32_t)lane * 64u;
+            if (!b3) {
+                // lines of 32 bytes or more: at most two newlines in a lane's 64 bytes
+                const uint32_t idx = (uint32_t)(__popc(b1 & lt_mask) + __popc(b2 & lt_mask));
+                nlc = (uint32_t)(__popc(b1) + __popc(b2));
+                if (c) {
+                    const uint32_t p1 = lo ? (uint32_t)(__ffs(lo) - 1) : 32u + (uint32_t)(__ffs(hi) - 1);
+                    if (idx < (uint32_t)SEGCAP) ent[idx] = (uint16_t)(pbase + p1);
+                    if (c >= 2u) {
+                        if (lo) lo &= lo - 1u; else hi &= hi - 1u;
+                        const uint32_t p2 = lo ? (uint32_t)(__ffs(lo) - 1) : 32u + (uint32_t)(__ffs(hi) - 1);
+                        if (idx + 1u < (uint32_t)SEGCAP) ent[idx + 1u] = (uint16_t)(pbase + p2);
+                    }
                 }
-            }
-        } else {
-            // short lines: exclusive scan of the per-lane counts, every lane walks its own newlines in order
-            uint32_t incl = c;
+            } else {
+                // short lines: exclusive scan of the per-lane counts, every lane walks its own newlines in order
+                uint32_t incl = c;
 #pragma unroll
-            for (int d = 1; d < 32; d <<= 1) {
-                const uint32_t o2 = __shfl_up_sync(0xffffffffu, incl, d);
-                if (lane >= d) incl += o2;
+                for (int d = 1; d < 32; d <<= 1) {
+                    const uint32_t o2 = __shfl_up_sync(0xffffffffu, incl, d);
+                    if (lane >= d) incl += o2;
+                }
+                nlc = __shfl_sync(0xffffffffu, incl, 31);
+                uint32_t idx = incl - c;
+                while (lo) { if (idx < (uint32_t)SEGCAP) ent[idx] = (uint16_t)(pbase + (uint32_t)(__ffs(lo) - 1)); lo &= lo - 1u; ++idx; }
+                while (hi) { if (idx < (uint32_t)SEGCAP) ent[idx] = (uint16_t)(pbase + 32u + (uint32_t)(__ffs(hi) - 1)); hi &= hi - 1u; ++idx; }
             }
-            nlc = __shfl_sync(0xffffffffu, incl, 31);
-            uint32_t idx = incl - c;
-            while (lo) { if (idx < (uint32_t)SEGCAP) ent[idx] = (uint16_t)(pbase + (uint32_t)(__ffs(lo) - 1)); lo &= lo - 1u; ++idx; }
-            while (hi) { if (idx < (uint32_t)SEGCAP) ent[idx] = (uint16_t)(pbase + 32u + (uint32_t)(__ffs(hi) - 1)); hi &= hi - 1u; ++idx; }
         }
-    }
-    __syncwarp();
+        __syncwarp();
     } else {
-    // ---- pass 1: positions, ranked in file order (chunk-major, lane-minor) ------------------
-    uint32_t m[4];
-    int cmax = 0;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-        s_data[warp * (REGION / 16) + j * 32 + lane] = v[j];
-        m[j] = chunk_eq_mask_r(v[j], k0a, k7f, k80);
-        cmax = max(cmax, __popc(m[j]));
-    }
-    const bool any2 = __any_sync(0xffffffffu, cmax >= 2);          // e.g. the "+" line of a FASTQ record
-    const bool multi = any2 && __any_sync(0xffffffffu, cmax >= 3);
-    if (!any2) {
-        // the usual FASTA case: no lane holds two newlines in its 16 bytes -> one ballot per chunk
+        // ---- pass 1: positions, ranked in file order (chunk-major, lane-minor) ------------------
+        uint32_t m[4];
+        int cmax = 0;
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
-            const uint32_t bn = __ballot_sync(0xffffffffu, m[j] != 0);
-            if (m[j]) {
-                const uint32_t idx = nlc + __popc(bn & lt_mask);
-                if (idx < (uint32_t)SEGCAP) ent[idx] = (uint16_t)(j * 512 + lane * 16 + chunk_bit_to_off(__ffs(m[j]) - 1));
-            }
-            nlc += __popc(bn);
+            s_data[warp * (REGION / 16) + j * 32 + lane] = v[j];
+            m[j] = chunk_eq_mask_r(v[j], k0a, k7f, k80);
+            cmax = max(cmax, __popc(m[j]));
         }
-    } else if (!multi) {
+        const bool any2 = __any_sync(0xffffffffu, cmax >= 2);          // e.g. the "+" line of a FASTQ record
+        const bool multi = any2 && __any_sync(0xffffffffu, cmax >= 3);
+        if (!any2) {
+            // the usual FASTA case: no lane holds two newlines in its 16 bytes -> one ballot per chunk
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            const int c = __popc(m[j]);
-            const uint32_t bn1 = __ballot_sync(0xffffffffu, c >= 1);
-            const uint32_t bn2 = __ballot_sync(0xffffffffu, c >= 2);
-            if (c) {
-                const uint32_t idx = nlc + __popc(bn1 & lt_mask) + __popc(bn2 & lt_mask);
-                const int xo = j * 512 + lane * 16;
-                int oa = chunk_bit_to_off(__ffs(m[j]) - 1);
-                if (c == 2) {
-                    const uint32_t m2 = m[j] & (m[j] - 1);
-                    const int ob = chunk_bit_to_off(__ffs(m2) - 1);
-                    const int hi = max(oa, ob);
-                    oa = min(oa, ob);
-                    if (idx + 1 < (uint32_t)SEGCAP) ent[idx + 1] = (uint16_t)(xo + hi);
+            for (int j = 0; j < 4; ++j) {
+                const uint32_t bn = __ballot_sync(0xffffffffu, m[j] != 0);
+                if (m[j]) {
+                    const uint32_t idx = nlc + __popc(bn & lt_mask);
+                    if (idx < (uint32_t)SEGCAP) ent[idx] = (uint16_t)(j * 512 + lane * 16 + chunk_bit_to_off(__ffs(m[j]) - 1));
                 }
-                if (idx < (uint32_t)SEGCAP) ent[idx] = (uint16_t)(xo + oa);
+                nlc += __popc(bn);
             }
-            nlc += __popc(bn1) + __popc(bn2);
-        }
-    }
-    if (multi) {
-        // short lines: three or more newlines inside one lane's 16 bytes -> shuffle scan per chunk, then each lane
-        // walks its own newlines in byte order (word, then byte within the word)
-        nlc = 0;
-#pragma unroll 1
-        for (int j = 0; j < 4; ++j) {
-            uint32_t mj = 0;
+        } else if (!multi) {
 #pragma unroll
-            for (int jj = 0; jj < 4; ++jj) if (jj == j) mj = m[jj];
-            const uint32_t c = (uint32_t)__popc(mj);
-            uint32_t incl = c;
-#pragma unroll
-            for (int d = 1; d < 32; d <<= 1) {
-                const uint32_t o2 = __shfl_up_sync(0xffffffffu, incl, d);
-                if (lane >= d) incl += o2;
-            }
-            uint32_t idx = nlc + incl - c;
-#pragma unroll 1
-            for (int w = 0; w < 4; ++w) {
-                uint32_t mw = mj & (0x80808080u >> w);
-                while (mw) {
-                    if (idx < (uint32_t)SEGCAP) ent[idx] = (uint16_t)(j * 512 + lane * 16 + chunk_bit_to_off(__ffs(mw) - 1));
-                    mw &= mw - 1;
-                    ++idx;
+            for (int j = 0; j < 4; ++j) {
+                const int c = __popc(m[j]);
+                const uint32_t bn1 = __ballot_sync(0xffffffffu, c >= 1);
+                const uint32_t bn2 = __ballot_sync(0xffffffffu, c >= 2);
+                if (c) {
+                    const uint32_t idx = nlc + __popc(bn1 & lt_mask) + __popc(bn2 & lt_mask);
+                    const int xo = j * 512 + lane * 16;
+                    int oa = chunk_bit_to_off(__ffs(m[j]) - 1);
+                    if (c == 2) {
+                        const uint32_t m2 = m[j] & (m[j] - 1);
+                        const int ob = chunk_bit_to_off(__ffs(m2) - 1);
+                        const int hi = max(oa, ob);
+                        oa = min(oa, ob);
+                        if (idx + 1 < (uint32_t)SEGCAP) ent[idx + 1] = (uint16_t)(xo + hi);
+                    }
+                    if (idx < (uint32_t)SEGCAP) ent[idx] = (uint16_t)(xo + oa);
                 }
+                nlc += __popc(bn1) + __popc(bn2);
             }
-            nlc += __shfl_sync(0xffffffffu, incl, 31);
         }
+        if (multi) {
+            // short lines: three or more newlines inside one lane's 16 bytes -> shuffle scan per chunk, then each lane
+            // walks its own newlines in byte order (word, then byte within the word)
+            nlc = 0;
+#pragma unroll 1
+            for (int j = 0; j < 4; ++j) {
+                uint32_t mj = 0;
+#pragma unroll
+                for (int jj = 0; jj < 4; ++jj) if (jj == j) mj = m[jj];
+                const uint32_t c = (uint32_t)__popc(mj);
+                uint32_t incl = c;
+#pragma unroll
+                for (int d = 1; d < 32; d <<= 1) {
+                    const uint32_t o2 = __shfl_up_sync(0xffffffffu, incl, d);
+                    if (lane >= d) incl += o2;
+                }
+                uint32_t idx = nlc + incl - c;
+#pragma unroll 1
+                for (int w = 0; w < 4; ++w) {
+                    uint32_t mw = mj & (0x80808080u >> w);
+                    while (mw) {
+                        if (idx < (uint32_t)SEGCAP) ent[idx] = (uint16_t)(j * 512 + lane * 16 + chunk_bit_to_off(__ffs(mw) - 1));
+                        mw &= mw - 1;
+                        ++idx;
+                    }
+                }
+                nlc += __shfl_sync(0xffffffffu, incl, 31);
+            }
+        }
+        __syncwarp();
     }
-    __syncwarp();
-    }   // pass-1 variant
 
     // ---- pass 2: one lane per newline: neighbour byte -> flag; counts; write-out --------------
     const uint8_t *sb = reinterpret_cast<const uint8_t *>(s_data + warp * (REGION / 16));
@@ -365,11 +309,10 @@ __global__ void __launch_bounds__(MARK_WARPS * 32, FXG_MARK_MINB) mark_kernel(co
         uint32_t imask = 0, hmask = 0;
         for (uint32_t k0 = 0; k0 < nround; k0 += 32) {
             const uint32_t k = k0 + lane;
-            uint32_t e = 0, cutv = 255u;
+            uint32_t e = 0;
             if (k < nlc) {
                 const uint32_t pos = ent[k];
                 e = pos;
-                if (FXG_MARK_CUT && MODE == 1 && pos + 2u < (uint32_t)REGION && region_byte<V>(sb, pos + 1u) == '@') cutv = name_cut_smem<V>(sb, pos + 2u);
                 if (MODE == 0) {
                     const uint32_t next = pos < (uint32_t)(REGION - 1) ? region_byte<V>(sb, pos + 1u)
                                                                       : (base + REGION < n ? (uint32_t)file[base + REGION] : 0u);
@@ -383,7 +326,7 @@ __global__ void __launch_bounds__(MARK_WARPS * 32, FXG_MARK_MINB) mark_kernel(co
                 const uint32_t hb = __ballot_sync(0xffffffffu, (e & E_HDR) != 0);
                 hc += __popc(hb);
                 if (k0 == 0) {
-                    // lines the lines kernel has to look at: header lines, the line after a header, and
+                    // lines fasta_lines_kernel has to look at: header lines, the line after a header, and
                     // lines whose length differs from the previous line's (k >= 2: all inside the region)
                     const uint32_t e1 = __shfl_up_sync(0xffffffffu, e, 1), e2 = __shfl_up_sync(0xffffffffu, e, 2);
                     const bool it = lane >= 2 && k < nlc &&
@@ -393,7 +336,6 @@ __global__ void __launch_bounds__(MARK_WARPS * 32, FXG_MARK_MINB) mark_kernel(co
                 }
             }
             if (k < nround) dst[k] = (uint16_t)e;
-            if (FXG_MARK_CUT && MODE == 1) P.cut[r * SEGCAP + k] = (uint8_t)cutv;   // one whole 32-byte sector per batch
             if (k < nlc) ent[k] = (uint16_t)e;                   // complete entries (for the region records)
         }
         __syncwarp();
@@ -406,7 +348,7 @@ __global__ void __launch_bounds__(MARK_WARPS * 32, FXG_MARK_MINB) mark_kernel(co
             }
         }
     } else {
-        // dense region: only the counts; the lines kernel re-reads the bytes
+        // dense region: only the counts; the rows kernels re-read the bytes
         if (MODE == 0) {
             uint32_t myh = 0;
             for (int x = lane; x < REGION; x += 32)
@@ -421,8 +363,6 @@ __global__ void __launch_bounds__(MARK_WARPS * 32, FXG_MARK_MINB) mark_kernel(co
             if (MODE == 0) P.rec2[r] = make_uint4(0u, 0xffffffffu, 0u, 0u);
         }
     }
-    __syncwarp();                                  // the warp's shared-memory buffers are reused by its next region
-    }   // regions of this warp
 }
 
 // =============================================================================================
@@ -794,85 +734,6 @@ __device__ __noinline__ unsigned long long full_region(const ScanParams *Pg, int
     return my_size;
 }
 
-constexpr int LG = 4;     // consecutive regions per warp of the lines kernel (all their loads in flight together)
-
-// Every line does work (FASTQ): one warp per LG regions, lane per line.
-template <int MODE>
-__global__ void __launch_bounds__(MARK_WARPS * 32) lines_kernel(const ScanParams P) {
-    const int64_t first_line = MODE == 1 ? P.totals->first_line : 0;   // global line phase, known only after the exchange
-    const int lane = threadIdx.x & 31;
-    const int64_t r0 = ((int64_t)blockIdx.x * MARK_WARPS + (threadIdx.x >> 5)) * LG;
-    if (r0 >= P.nreg) return;
-    unsigned long long my_size = 0;                // FASTQ: sum of rlen seen by this thread
-
-    // everything this warp needs, requested at once: the records of its LG regions and the 32 - LG regions
-    // before them (lane l <-> region r0 + LG-1 - l), the exclusive prefixes, the first 64 entries of each segment
-    const int64_t rq = r0 + (LG - 1) - lane;
-    const uint2 A = rq >= 0 ? P.rc[rq] : make_uint2(0u, 0u);       // rc is zero padded past nreg
-    ulonglong2 X[LG];
-    uint32_t E[LG][2];
-#pragma unroll
-    for (int i = 0; i < LG; ++i) {
-        const int64_t r = r0 + i;
-        X[i] = make_ulonglong2(0, 0); E[i][0] = E[i][1] = 0;
-        if (r < P.nreg) {
-            X[i] = P.ex[r];
-            E[i][0] = P.seg[r * SEGCAP + lane];          // speculative: entries past the count are never used
-            E[i][1] = P.seg[r * SEGCAP + 32 + lane];
-        }
-    }
-    const uint32_t cntl = A.x & 0xffffu;
-    const uint32_t nzall = __ballot_sync(0xffffffffu, cntl != 0);
-    const bool window_hits_start = r0 + (LG - 1) - 31 <= 0;         // no region before the window
-
-#pragma unroll
-    for (int i = 0; i < LG; ++i) {
-        const int64_t r = r0 + i;
-        const int me = LG - 1 - i;                                    // the lane holding region r's record
-        const int nl = (int)__shfl_sync(0xffffffffu, cntl, me);
-        if (nl == 0) continue;
-
-        // ---- the two newlines before the region, from the records of the regions before it ----
-        Prev2 cy;
-        cy.pos1 = cy.pos0 = NOPOS; cy.h1 = cy.h0 = 0;
-        {
-            bool slow = false;
-            const uint32_t nz = nzall & ~((2u << me) - 1u);           // non-empty regions before r
-            if (nz) {
-                const int f1 = __ffs(nz) - 1;
-                const uint32_t n1 = __shfl_sync(0xffffffffu, cntl, f1), y1 = __shfl_sync(0xffffffffu, A.y, f1);
-                const int64_t b1 = (r0 + (LG - 1) - f1) * REGION;
-                if (n1 > (uint32_t)SEGCAP) slow = true;
-                else {
-                    cy.pos1 = b1 + (y1 & E_POS); cy.h1 = (y1 >> 15) & 1u;
-                    if (n1 >= 2) { cy.pos0 = b1 + ((y1 >> 16) & E_POS); cy.h0 = y1 >> 31; }
-                    else {
-                        const uint32_t nz2 = nz & ~(1u << f1);
-                        if (nz2) {
-                            const int f2 = __ffs(nz2) - 1;
-                            const uint32_t n2 = __shfl_sync(0xffffffffu, cntl, f2), y2 = __shfl_sync(0xffffffffu, A.y, f2);
-                            if (n2 > (uint32_t)SEGCAP) slow = true;
-                            else { cy.pos0 = (r0 + (LG - 1) - f2) * REGION + (y2 & E_POS); cy.h0 = (y2 >> 15) & 1u; }
-                        } else if (window_hits_start) { cy.pos0 = -1; cy.h0 = is_hdr_at<MODE>(P, 0); }
-                        else slow = true;
-                    }
-                }
-            } else if (window_hits_start) { cy.pos1 = -1; cy.h1 = is_hdr_at<MODE>(P, 0); }
-            else slow = true;
-            if (slow) cy = carry_walk<MODE>(P.self, r);
-            if (MODE != 0) cy.h1 = cy.h0 = 0;
-        }
-        if (nl <= SEGCAP) region_batches<MODE>(P, first_line, r, nl, cy, X[i], E[i][0], E[i][1], my_size);
-        else my_size += dense_region<MODE>(P.self, first_line, r, cy, X[i]);
-    }
-
-    if (MODE == 1) {
-#pragma unroll
-        for (int d = 16; d > 0; d >>= 1) my_size += (unsigned long long)shfl_down_i64((int64_t)my_size, d);
-        if (lane == 0 && my_size) atomicAdd((unsigned long long *)&P.totals->sum_len, my_size);
-    }
-}
-
 // FASTQ fast path: one LANE per read.  A warp takes RG consecutive regions, flattens their newline lists
 // (plus two look-ahead regions) into shared memory, and every lane assembles the whole 32-byte row of one
 // read from five consecutive newline positions -- straight-line code, one row store, the name cut searched
@@ -880,19 +741,12 @@ __global__ void __launch_bounds__(MARK_WARPS * 32) lines_kernel(const ScanParams
 // of a read that began earlier are written field by field) and completes the reads that START in its span
 // as far as its window reaches; lines past the window are (also) covered by the warp that owns their
 // region, which writes identical values.  Spans containing a dense region use the general path.
-#ifndef FXG_FQ_PRELOAD
-#define FXG_FQ_PRELOAD 0
-#endif
-#ifndef FXG_FQ_PAIRSTORE
-#define FXG_FQ_PAIRSTORE 1
-#endif
 constexpr int RG = 8;                          // regions per warp
 constexpr int RWIN = RG + 2;                   // + look-ahead
 static_assert(RWIN * REGION <= 32768, "window positions must fit 15 bits");
 
 __global__ void __launch_bounds__(MARK_WARPS * 32) fastq_records_kernel(const ScanParams Pin) {
     __shared__ uint16_t s_flat[MARK_WARPS][RWIN * SEGCAP];      // position in window | '\r' before << 15
-    __shared__ uint8_t  s_cut[MARK_WARPS][FXG_MARK_CUT ? RWIN * SEGCAP : 1];   // name cut of the line after that newline (mark)
     const ScanParams &P = Pin;
     const int64_t first_line = Pin.totals->first_line;          // global line phase, known only after the exchange
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -915,16 +769,7 @@ __global__ void __launch_bounds__(MARK_WARPS * 32) fastq_records_kernel(const Sc
         const uint64_t ex0 = (uint64_t)shfl_i64((int64_t)exl, 1);    // lines before the span
         // ---- flatten the window ----
         uint16_t *flat = s_flat[warp];
-        uint8_t *cutf = s_cut[warp];
-        // Entries of all window regions are requested BEFORE any of them is used: two entries per lane and load
-        // (64 per region cover every region of a typical short-read file in one load), RWIN loads in flight together
-        // instead of RWIN dependent round trips.  Entries past a region's count are stale and never used.
-        uint32_t E2[RWIN];
-#pragma unroll
-        for (int i = 0; i < RWIN; ++i) {
-            E2[i] = 0u;
-            if (FXG_FQ_PRELOAD && r0 + i < P.nreg) E2[i] = reinterpret_cast<const uint32_t *>(P.seg + (r0 + i) * SEGCAP)[lane];
-        }
+        // Two entries per lane and load: 64 per region cover every region of a typical short-read file in one load.
         int W = 0, Ls = 0;                                           // entries in the window / in the span
         bool closed = false;                                         // a dense look-ahead region ends the window
 #pragma unroll
@@ -933,8 +778,8 @@ __global__ void __launch_bounds__(MARK_WARPS * 32) fastq_records_kernel(const Sc
             if (nl > SEGCAP) closed = true;
             if (!closed) {
                 const int k = 2 * lane;
-                if (!FXG_FQ_PRELOAD && k < nl) E2[i] = reinterpret_cast<const uint32_t *>(P.seg + (r0 + i) * SEGCAP)[lane];
-                const uint32_t e0 = E2[i] & 0xffffu, e1 = E2[i] >> 16;
+                const uint32_t E2 = k < nl ? reinterpret_cast<const uint32_t *>(P.seg + (r0 + i) * SEGCAP)[lane] : 0u;
+                const uint32_t e0 = E2 & 0xffffu, e1 = E2 >> 16;
                 if (k < nl) flat[W + k] = (uint16_t)((i * REGION + (int)(e0 & E_POS)) | ((e0 & E_CR) ? 0x8000u : 0u));
                 if (k + 1 < nl) flat[W + k + 1] = (uint16_t)((i * REGION + (int)(e1 & E_POS)) | ((e1 & E_CR) ? 0x8000u : 0u));
                 if (nl > 64) {                                       // lines shorter than 32 bytes on average
@@ -944,10 +789,6 @@ __global__ void __launch_bounds__(MARK_WARPS * 32) fastq_records_kernel(const Sc
                         flat[W + kk] = (uint16_t)((i * REGION + (int)(e & E_POS)) | ((e & E_CR) ? 0x8000u : 0u));
                     }
                 }
-                if (FXG_MARK_CUT) {
-                    const uint8_t *cg = P.cut + (r0 + i) * SEGCAP;
-                    for (int kk = lane; kk < nl; kk += 32) cutf[W + kk] = cg[kk];
-                }
                 W += nl;
             }
             if (i == RG - 1) Ls = W;
@@ -955,14 +796,11 @@ __global__ void __launch_bounds__(MARK_WARPS * 32) fastq_records_kernel(const Sc
         __syncwarp();
         // ---- the newline before the span ----
         int64_t carry;
-        uint32_t carry_cut = 255u;                                   // cut of the line that starts right after `carry`
         {
             const uint32_t pn = __shfl_sync(0xffffffffu, nll, 0), py = __shfl_sync(0xffffffffu, rec.y, 0);
             if (r0 == 0) carry = -1;
-            else if (pn >= 1 && pn <= (uint32_t)SEGCAP) {
-                carry = (r0 - 1) * REGION + (int64_t)(py & E_POS);
-                if (FXG_MARK_CUT) carry_cut = P.cut[(r0 - 1) * SEGCAP + (pn - 1)];
-            } else carry = carry_walk<1>(P.self, r0).pos1;
+            else if (pn >= 1 && pn <= (uint32_t)SEGCAP) carry = (r0 - 1) * REGION + (int64_t)(py & E_POS);
+            else carry = carry_walk<1>(P.self, r0).pos1;
         }
         const int64_t span_base = r0 * REGION;
         auto POS = [&](int f) -> int64_t { return f < 0 ? carry : span_base + (int64_t)(flat[f] & 0x7fffu); };
@@ -1002,10 +840,7 @@ __global__ void __launch_bounds__(MARK_WARPS * 32) fastq_records_kernel(const Sc
                 if (l > 0 && CR(f)) --l;
                 if (l < 0) l = 0;
                 const int64_t s = pm1 + 1;
-                const uint32_t cv = !FXG_MARK_CUT ? 255u : (f >= 1 ? (uint32_t)cutf[f - 1] : carry_cut);   // found by mark while the bytes were on chip
-                if (cv < 254u) k = (int64_t)cv < l ? (int64_t)cv : l;
-                else if (cv == 254u) k = l;
-                else if (s + 1 + l + 20 <= P.capacity) {
+                if (s + 1 + l + 20 <= P.capacity) {
                     int which;
                     k = find_first_of2(file + s + 1, l, 0x20202020u, 0x00000000u, &which);
                     if (which == 2) k = l;          // a NUL before any space: strchr() finds nothing (fastq.c:112)
@@ -1030,7 +865,7 @@ __global__ void __launch_bounds__(MARK_WARPS * 32) fastq_records_kernel(const Sc
             //      that each instruction writes whole sectors: lanes (2j, 2j+1) write row 2j, then row 2j+1. ----
             const bool full = mine && have3 && row < P.qrows_cap;
             const int other_full = __shfl_xor_sync(0xffffffffu, full ? 1 : 0, 1);   // every lane must reach the shuffle
-            const bool pair_full = FXG_FQ_PAIRSTORE && full && other_full != 0;
+            const bool pair_full = full && other_full != 0;
             longlong2 a, b;
             a.x = soff; a.y = qoff;
             b.x = rlen; b.y = (long long)(((unsigned long long)(uint32_t)(int)k << 32) | (uint32_t)(int)len);
@@ -1336,7 +1171,6 @@ static int scan_params(fxg_ctx *ctx, const fxg_file *f, int mode, int64_t base_o
         if ((rc = ctx->counters.reserve(1024))) return rc;
         if ((rc = ctx->tile_desc.reserve(off_r2 + (mode == 0 ? (size_t)nreg * sizeof(uint4) : 0)))) return rc;
         if ((rc = ctx->seg.reserve((size_t)nreg * SEGCAP * sizeof(uint16_t)))) return rc;
-        if (FXG_MARK_CUT && mode == 1 && (rc = ctx->cut.reserve((size_t)nreg * SEGCAP))) return rc;
         const int64_t want = guess_rows(mode, n);
         if (mode == 0) {
             if (ctx->row_tmp.cap < (size_t)(want + 2) * sizeof(FastaTmp) && (rc = ctx->row_tmp.reserve((size_t)(want + 2) * sizeof(FastaTmp)))) return rc;
@@ -1354,7 +1188,6 @@ static int scan_params(fxg_ctx *ctx, const fxg_file *f, int mode, int64_t base_o
     P.ex = (ulonglong2 *)((uint8_t *)ctx->tile_desc.ptr + off_ex);
     P.rec2 = (uint4 *)((uint8_t *)ctx->tile_desc.ptr + off_r2);
     P.seg = (uint16_t *)ctx->seg.ptr;
-    P.cut = (uint8_t *)ctx->cut.ptr;
     P.totals = (ScanTotals *)((uint8_t *)ctx->counters.ptr + 64);
     *tmp_slots = 0;
     if (mode == 0) {
@@ -1386,11 +1219,12 @@ extern "C" int fxg_scan_begin(fxg_ctx *ctx, const fxg_file *f, int mode, int64_t
     const int64_t nb = (nreg + PS_BLOCK - 1) / PS_BLOCK, nreg_pad = nb * PS_BLOCK;
     FXG_CUDA(cudaMemsetAsync(ctx->counters.ptr, 0, 1024, ctx->stream));
     if (nreg_pad > nreg) FXG_CUDA(cudaMemsetAsync(P.rc + nreg, 0, (size_t)(nreg_pad - nreg) * 8, ctx->stream));
-    const unsigned grid = (unsigned)((nreg + (int64_t)MARK_WARPS * FXG_MARK_RPW - 1) / ((int64_t)MARK_WARPS * FXG_MARK_RPW));
+    const unsigned grid = (unsigned)((nreg + MARK_WARPS - 1) / MARK_WARPS);
     {
         FxgProfScope prof(ctx, FXG_PROF_SCAN);
-        if (mode == 0) mark_kernel<0, FXG_MARK_V_FASTA><<<grid, MARK_WARPS * 32, 0, ctx->stream>>>(P);
-        else mark_kernel<1, FXG_MARK_V_FASTQ><<<grid, MARK_WARPS * 32, 0, ctx->stream>>>(P);
+        // pass-1 variant per format: V1 is the faster one for FASTA, V2 for FASTQ (DESIGN.md section 3)
+        if (mode == 0) mark_kernel<0, 1><<<grid, MARK_WARPS * 32, 0, ctx->stream>>>(P);
+        else mark_kernel<1, 2><<<grid, MARK_WARPS * 32, 0, ctx->stream>>>(P);
     }
     FXG_CUDA(cudaGetLastError());
     {
@@ -1426,9 +1260,6 @@ static int launch_phase_b(fxg_ctx *ctx, const ScanParams &P0, int mode, int64_t 
         if (mode == 0) {
             const unsigned lgrid = (unsigned)((nreg + MARK_WARPS * 32 - 1) / (MARK_WARPS * 32));
             fasta_lines_kernel<<<lgrid, MARK_WARPS * 32, 0, ctx->stream>>>(P);
-        } else if (getenv("FXG_FASTQ_LINES_GENERIC")) {      // lane-per-line path for every region (A/B, debugging)
-            const unsigned lgrid = (unsigned)((nreg + MARK_WARPS * LG - 1) / (MARK_WARPS * LG));
-            lines_kernel<1><<<lgrid, MARK_WARPS * 32, 0, ctx->stream>>>(P);
         } else {
             const unsigned lgrid = (unsigned)((nreg + MARK_WARPS * RG - 1) / (MARK_WARPS * RG));
             fastq_records_kernel<<<lgrid, MARK_WARPS * 32, 0, ctx->stream>>>(P);

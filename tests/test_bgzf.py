@@ -82,18 +82,6 @@ def test_gpu_inflate_matches_zlib(kind):
 
 
 @pytest.mark.gpu
-def test_warp_per_member_kernel_still_agrees(monkeypatch):
-    """the earlier warp-per-member inflate kernel (A/B switch) decodes the same bytes"""
-    from pyfastx_b200 import engine
-    monkeypatch.setenv("FXG_INFLATE_WARP_PER_MEMBER", "1")
-    eng = engine.get_engine(0)
-    for data, level in ((synth.synth_fasta(300, seed=11), 6), (synth.synth_fastq(8000, seed=3), 1)):
-        f = eng.stage_bgzf(np.frombuffer(bgzf_compress(data, level), dtype=np.uint8))
-        assert f.download().tobytes() == data
-        f.free()
-
-
-@pytest.mark.gpu
 def test_corrupt_member_is_reported():
     from pyfastx_b200 import engine
     eng = engine.get_engine(0)
