@@ -3,7 +3,7 @@
 // Replaces the per-line loops of pyfastx_create_index (reference src/index.c:226-361) and
 // pyfastx_fastq_create_index (src/fastq.c:84-171), both driven by ks_getuntil2
 // (src/kseq.c:59-109).  The file bytes resident in HBM are read ONCE; everything after that
-// works on a compact newline list (2 bytes per line, ~3 % of the file for 80-column FASTA).
+// works on compact per-region records (newline lists, FASTA line facts).
 //
 // Design (see DESIGN.md section 3):
 //   mark    one warp per 2 KiB region, no communication between warps at all: 4 coalesced
@@ -12,7 +12,8 @@
 //           {position in region | '\r' before | '>' after}, plus the region's counts
 //           {#newlines, #header starts}.  This kernel carries all of the file traffic and is
 //           a pure stream: nothing in it waits on another CTA.
-//   prefix  exclusive prefix of the region counts (three small kernels over 4 bytes per region).
+//   prefix  exclusive prefix of the region counts (small kernels over 4 bytes per region; FASTA keeps
+//           block sums only).
 //   rows    reads only the newline list (and the file bytes of header / read-name lines).  Every
 //           quantity the reference carries from line to line is re-expressed as a local rule on
 //           (this line, previous line, global line index, global header ordinal):
@@ -20,10 +21,13 @@
 //             - a sequence line that follows a header writes llen;
 //             - a sequence line whose length differs from the previous sequence line raises an
 //               "event" (count, min/max line index, sum of length deltas) on its record.
-//           FASTA (fasta_lines_kernel): one lane per region walks only the lines that matter, found
-//           from the records mark left behind; a tiny finalize kernel then derives blen, slen, norm
-//           per record from neighbouring headers and the event summary (proof of equivalence with
-//           index.c:325-342 in DESIGN.md).
+//           FASTA: mark itself settles every line k >= 2 of a region that changes a record into a line
+//           fact (name cut included), and writes the newline list only for general regions (more than
+//           32 newlines or 3 facts).  fasta_rows_kernel scans the region counts per CTA (no per-region
+//           prefix array), resolves lines 0 and 1 of each region from the region before it and applies
+//           the facts; fasta_general_kernel runs the general regions from their newline list; a tiny
+//           finalize kernel then derives blen, slen, norm per record from neighbouring headers and the
+//           event summary (proof of equivalence with index.c:325-342 in DESIGN.md).
 //           FASTQ (fastq_records_kernel): no per-record state at all, line k of the file writes
 //           field k%4 of row k/4; one lane builds the whole row of a read from five consecutive
 //           newline positions, and reads the name line once to find the name cut.
@@ -48,6 +52,16 @@ constexpr int MARK_WARPS = 8;             // warps per CTA of the mark / rows ke
 constexpr int PS_THREADS = 256, PS_PER_THREAD = 16, PS_BLOCK = PS_THREADS * PS_PER_THREAD;   // regions per prefix block
 constexpr int64_t NOPOS = INT64_MIN / 4;
 constexpr uint32_t E_POS = 0x07ffu, E_CR = 1u << 14, E_HDR = 1u << 15;
+// FASTA region record.  Every region keeps its first two entries (fw); bits 11..13 of the first entry are free and
+// carry the number of line facts (FW_NF) or FW_GEN: the region is settled by full_region from its newline list.
+// A line fact describes one line k >= 2 of the region that changes a record (a header, the first sequence line
+// after a header, a change of line length):
+//   x = newline position | k << 11 | header starts before entry k << 16 | kind << 21
+//   y = LF_HDR: dlen | nlen << 11 | (elen - 1) << 22 | LF_CUT_UNKNOWN;  LF_LLEN: len + 1;  LF_EVENT: change of len
+constexpr uint32_t FW_NF_SHIFT = 11, FW_NF = 3u << FW_NF_SHIFT, FW_GEN = 1u << 13;
+constexpr int LF_MAX = 3, LF_STRIDE = 4;  // facts per region; uint2 slots per region (32 bytes)
+constexpr uint32_t LF_HDR = 0, LF_LLEN = 1, LF_EVENT = 2, LF_CUT_UNKNOWN = 1u << 23;
+constexpr uint32_t NAME_SCAN = 64;        // header bytes mark searches for the name cut
 
 struct __align__(16) FastaTmp {   // per header slot (slot 0 = lines before the first header)
     int64_t  boff;       // header thread
@@ -90,9 +104,12 @@ struct ScanParams {
     int       flags;
     uint2    *rc;           // per region: {newlines | header starts << 16, last entry | the one before << 16}
                             // (padded to PS_BLOCK with zeros)
-    uint4    *rec2;         // FASTA, per region: {first entry | second << 16, interesting-line mask, header mask, 0}
-    uint16_t *seg;          // per region: SEGCAP entries, file order
-    ulonglong2 *ex;         // per region: exclusive {newlines, header starts}
+    uint32_t *fw;           // FASTA, per region: first entry | second << 16, FW_* flags in the first (padded to PS_BLOCK)
+    uint2    *lf;           // FASTA, per region: up to LF_MAX line facts (written only where FW_NF is not 0);
+                            // a general region's slot holds its exclusive {newlines, header starts} instead
+    uint32_t *gblk;         // FASTA, per prefix block: 1 if it has a general region (fasta_rows_kernel)
+    uint16_t *seg;          // per region: SEGCAP entries, file order (FASTA: general regions only)
+    ulonglong2 *ex;         // FASTQ, per region: exclusive {newlines, header starts}
     ulonglong2 *bs;         // per prefix block
     ScanTotals *totals;
     FastaTmp *tmp;          // FASTA
@@ -306,7 +323,8 @@ __global__ void __launch_bounds__(MARK_WARPS * 32, FXG_MARK_MINB) mark_kernel(co
     if (nlc <= (uint32_t)SEGCAP) {
         uint16_t *dst = P.seg + r * SEGCAP;
         const uint32_t nround = (nlc + 15u) & ~15u;         // whole 32-byte sectors, zero padded
-        uint32_t imask = 0, hmask = 0;
+        bool general = MODE == 1 || nlc > 32u;              // FASTA writes the newline list of general regions only
+        uint32_t nfacts = 0;
         for (uint32_t k0 = 0; k0 < nround; k0 += 32) {
             const uint32_t k = k0 + lane;
             uint32_t e = 0;
@@ -326,16 +344,47 @@ __global__ void __launch_bounds__(MARK_WARPS * 32, FXG_MARK_MINB) mark_kernel(co
                 const uint32_t hb = __ballot_sync(0xffffffffu, (e & E_HDR) != 0);
                 hc += __popc(hb);
                 if (k0 == 0) {
-                    // lines fasta_lines_kernel has to look at: header lines, the line after a header, and
-                    // lines whose length differs from the previous line's (k >= 2: all inside the region)
+                    // lines that change a record: header lines, the line after a header, and lines whose length
+                    // differs from the previous line's.  k >= 2: the line and both newlines before it lie in the
+                    // region, so it is settled here, one lane per line, into a line fact.
                     const uint32_t e1 = __shfl_up_sync(0xffffffffu, e, 1), e2 = __shfl_up_sync(0xffffffffu, e, 2);
-                    const bool it = lane >= 2 && k < nlc &&
-                                    (((e1 | e2) & E_HDR) != 0 || (e & E_POS) - (e1 & E_POS) != (e1 & E_POS) - (e2 & E_POS));
-                    imask = __ballot_sync(0xffffffffu, it);
-                    hmask = hb;
+                    const uint32_t p = e & E_POS, p1 = e1 & E_POS, L = p - p1, dL = L - (p1 - (e2 & E_POS));
+                    const bool it = lane >= 2 && k < nlc && (((e1 | e2) & E_HDR) != 0 || dL != 0u);
+                    const uint32_t imask = __ballot_sync(0xffffffffu, it);
+                    nfacts = (uint32_t)__popc(imask);
+                    general |= nfacts > (uint32_t)LF_MAX;
+                    if (!general) {
+                        uint32_t kind = LF_EVENT, y = dL;
+                        if (e1 & E_HDR) {
+                            const uint32_t elen = region_byte<V>(sb, p - 1u) == '\r' ? 2u : 1u, dlen = L - 1u - elen;
+                            kind = LF_HDR;
+                            y = dlen | (dlen << 11) | ((elen - 1u) << 22);
+                        } else if (e2 & E_HDR) {
+                            kind = LF_LLEN;
+                            y = L;
+                        }
+                        // the name cut: first ' ' or '\t' of the header, all lanes testing its bytes at once
+                        uint32_t hm = __ballot_sync(0xffffffffu, it && kind == LF_HDR && !(P.flags & FXG_SCAN_FULL_NAME));
+                        while (hm) {
+                            const int f = __ffs(hm) - 1;
+                            hm &= hm - 1u;
+                            const uint32_t s1 = __shfl_sync(0xffffffffu, p1 + 2u, f), dlen = __shfl_sync(0xffffffffu, y & E_POS, f);
+                            const uint32_t lim = min(dlen, NAME_SCAN);
+                            uint32_t cut = dlen > NAME_SCAN ? ~0u : dlen;
+                            for (uint32_t o = 0; o < lim; o += 32) {
+                                const uint32_t b = o + lane < lim ? region_byte<V>(sb, s1 + o + lane) : 0u;
+                                const uint32_t m = __ballot_sync(0xffffffffu, b == ' ' || b == '\t');
+                                if (m) { cut = o + (uint32_t)(__ffs(m) - 1); break; }
+                            }
+                            if (lane == f) y = cut == ~0u ? (y | LF_CUT_UNKNOWN) : ((y & ~(E_POS << 11)) | (cut << 11));
+                        }
+                        if (it)
+                            P.lf[r * LF_STRIDE + __popc(imask & lt_mask)] =
+                                make_uint2(p | ((uint32_t)k << 11) | ((uint32_t)__popc(hb & lt_mask) << 16) | (kind << 21), y);
+                    }
                 }
             }
-            if (k < nround) dst[k] = (uint16_t)e;
+            if (general && k < nround) dst[k] = (uint16_t)e;
             if (k < nlc) ent[k] = (uint16_t)e;                   // complete entries (for the region records)
         }
         __syncwarp();
@@ -344,7 +393,7 @@ __global__ void __launch_bounds__(MARK_WARPS * 32, FXG_MARK_MINB) mark_kernel(co
             P.rc[r] = make_uint2(nlc | (hc << 16), last | (prev << 16));
             if (MODE == 0) {
                 const uint32_t f0 = nlc >= 1 ? ent[0] : 0u, f1 = nlc >= 2 ? ent[1] : 0u;
-                P.rec2[r] = make_uint4(f0 | (f1 << 16), nlc > 32u ? 0xffffffffu : imask, hmask, 0u);
+                P.fw[r] = f0 | (f1 << 16) | (general ? FW_GEN : nfacts << FW_NF_SHIFT);
             }
         }
     } else {
@@ -360,7 +409,7 @@ __global__ void __launch_bounds__(MARK_WARPS * 32, FXG_MARK_MINB) mark_kernel(co
         }
         if (lane == 0) {
             P.rc[r] = make_uint2(nlc | (hc << 16), 0u);
-            if (MODE == 0) P.rec2[r] = make_uint4(0u, 0xffffffffu, 0u, 0u);
+            if (MODE == 0) P.fw[r] = FW_GEN;
         }
     }
 }
@@ -503,6 +552,43 @@ __device__ __forceinline__ bool nl_at(const ScanParams &P, int64_t x) {         
     return x < P.n ? P.file[x] == '\n' : (x == P.n && P.n > 0 && P.file[P.n - 1] != '\n');
 }
 
+// ---- FASTA record slot updates, shared by the line walk (do_line) and the line facts ----
+// name length: bytes of the header line starting at s (its '>') before the first ' ' or '\t'
+__device__ __forceinline__ int64_t fasta_name_len(const ScanParams &P, int64_t s, int64_t dlen) {
+    int64_t nlen = 0;
+    if (s + 1 + dlen + 20 <= P.capacity) {
+        int which;
+        nlen = find_first_of2(P.file + s + 1, dlen, 0x20202020u, 0x09090909u, &which);
+    } else {
+        while (nlen < dlen) {
+            const uint8_t ch = P.file[s + 1 + nlen];
+            if (ch == ' ' || ch == '\t') break;
+            ++nlen;
+        }
+    }
+    return nlen;
+}
+// header line ending in the newline at p
+__device__ __forceinline__ void fasta_header(const ScanParams &P, int64_t slot, int64_t p, int64_t lineidx, int64_t dlen,
+                                             int64_t nlen, int elen) {
+    if (slot < P.tmp_cap) {
+        FastaTmp *t = &P.tmp[slot];
+        t->boff = P.base_offset + p + 1;
+        t->lineidx = lineidx;
+        t->dlen = (int32_t)dlen;
+        t->nlen = (int32_t)nlen;
+        t->elen = (uint32_t)elen;
+    }
+}
+// sequence line whose length differs from the previous sequence line's by dL (slot < tmp_cap)
+__device__ __forceinline__ void fasta_event(const ScanParams &P, int64_t slot, int64_t lineidx, int64_t dL) {
+    FastaTmp *t = &P.tmp[slot];
+    atomicAdd(&t->D, 1u);
+    atomicMax((unsigned long long *)&t->evmax, (unsigned long long)lineidx);
+    atomicMax((unsigned long long *)&t->evminc, ~(unsigned long long)lineidx);
+    atomicAdd((unsigned long long *)&t->S, (unsigned long long)dL);
+}
+
 // ---- one line: newline at p, previous newlines pm1, pm2; h1 / h2: the line starting after pm1 / pm2 is a
 //      header; hcount: header starts up to and including the one after pm1 (= record ordinal + 1);
 //      cr: the byte before p is '\r' (FASTQ entries carry it; FASTA looks it up for header lines only) ----
@@ -517,41 +603,15 @@ __device__ __forceinline__ void do_line(const ScanParams &P, int64_t first_line,
         if (h1) {
             const int elen = (p >= 1 && (p - 1 < P.n ? file[p - 1] : 0) == '\r') ? 2 : 1;
             const int64_t dlen = L - 1 - elen;
-            int64_t nlen = dlen;
-            if (!(P.flags & FXG_SCAN_FULL_NAME)) {
-                nlen = 0;
-                if (s + 1 + dlen + 20 <= P.capacity) {
-                    int which;
-                    nlen = find_first_of2(file + s + 1, dlen, 0x20202020u, 0x09090909u, &which);
-                } else {
-                    while (nlen < dlen) {
-                        const uint8_t ch = file[s + 1 + nlen];
-                        if (ch == ' ' || ch == '\t') break;
-                        ++nlen;
-                    }
-                }
-            }
-            if (slot < P.tmp_cap) {
-                FastaTmp *t = &P.tmp[slot];
-                t->boff = P.base_offset + p + 1;
-                t->lineidx = lineidx;
-                t->dlen = (int32_t)dlen;
-                t->nlen = (int32_t)nlen;
-                t->elen = (uint32_t)elen;
-            }
+            const int64_t nlen = (P.flags & FXG_SCAN_FULL_NAME) ? dlen : fasta_name_len(P, s, dlen);
+            fasta_header(P, slot, p, lineidx, dlen, nlen, elen);
         } else if (slot < P.tmp_cap) {
             const bool prev_exists = pm1 >= 0;
             if (!prev_exists || h2) {
                 P.tmp[slot].llen = L;
             } else {
                 const int64_t prevL = pm1 - pm2;
-                if (L != prevL) {
-                    FastaTmp *t = &P.tmp[slot];
-                    atomicAdd(&t->D, 1u);
-                    atomicMax((unsigned long long *)&t->evmax, (unsigned long long)lineidx);
-                    atomicMax((unsigned long long *)&t->evminc, ~(unsigned long long)lineidx);
-                    atomicAdd((unsigned long long *)&t->S, (unsigned long long)(L - prevL));
-                }
+                if (L != prevL) fasta_event(P, slot, lineidx, L - prevL);
             }
         }
     } else {
@@ -611,11 +671,9 @@ __device__ __noinline__ Prev2 carry_walk(const ScanParams *Pg, int64_t r) {
         q -= f;
         const int cq = (int)__shfl_sync(0xffffffffu, c, f);
         if (cq <= SEGCAP) {
-            const uint16_t *sg = P.seg + q * SEGCAP;
-            for (int i = cq - 1; i >= 0 && need > 0; --i) {
-                const uint32_t e = sg[i];
-                push(q * REGION + (int64_t)(e & E_POS), MODE == 0 ? (e >> 15) : 0u);
-            }
+            const uint32_t y = P.rc[q].y;                      // the region's last entry | the one before << 16
+            push(q * REGION + (int64_t)(y & E_POS), MODE == 0 ? ((y >> 15) & 1u) : 0u);
+            if (need > 0 && cq >= 2) push(q * REGION + (int64_t)((y >> 16) & E_POS), MODE == 0 ? (y >> 31) : 0u);
         } else {
             for (int64_t x = q * REGION + REGION - 1; x >= q * REGION && need > 0; --x)
                 if (nl_at(P, x)) push(x, is_hdr_at<MODE>(P, x + 1));
@@ -719,14 +777,14 @@ __device__ __forceinline__ void region_batches(const ScanParams &P, int64_t firs
 }
 
 // ---- general path for one region: everything looked up from scratch ----
+// X: exclusive {newlines, header starts} of the region
 template <int MODE>
-__device__ __noinline__ unsigned long long full_region(const ScanParams *Pg, int64_t first_line, int64_t r) {
+__device__ __noinline__ unsigned long long full_region(const ScanParams *Pg, int64_t first_line, int64_t r, ulonglong2 X) {
     const ScanParams &P = *Pg;
     unsigned long long my_size = 0;
     const int lane = threadIdx.x & 31;
     const int nl = (int)(P.rc[r].x & 0xffffu);
     if (nl == 0) return 0;
-    const ulonglong2 X = P.ex[r];
     Prev2 cy = carry_walk<MODE>(Pg, r);
     if (MODE != 0) cy.h1 = cy.h0 = 0;
     if (nl <= SEGCAP) region_batches<MODE>(P, first_line, r, nl, cy, X, P.seg[r * SEGCAP + lane], P.seg[r * SEGCAP + 32 + lane], my_size);
@@ -764,7 +822,7 @@ __global__ void __launch_bounds__(MARK_WARPS * 32) fastq_records_kernel(const Sc
     const uint32_t densem = __ballot_sync(0xffffffffu, nll > (uint32_t)SEGCAP);
     if (densem & (((1u << RG) - 1u) << 1)) {                       // a dense region inside the span
         for (int i = 0; i < RG; ++i)
-            if (r0 + i < P.nreg) my_size += full_region<1>(P.self, first_line, r0 + i);
+            if (r0 + i < P.nreg) my_size += full_region<1>(P.self, first_line, r0 + i, P.ex[r0 + i]);
     } else {
         const uint64_t ex0 = (uint64_t)shfl_i64((int64_t)exl, 1);    // lines before the span
         // ---- flatten the window ----
@@ -895,60 +953,110 @@ __global__ void __launch_bounds__(MARK_WARPS * 32) fastq_records_kernel(const Sc
     if (lane == 0 && my_size) atomicAdd((unsigned long long *)&P.totals->sum_len, my_size);
 }
 
-// FASTA: almost no line does work (only header lines, the line after a header, and lines whose length
-// differs from the previous line's).  One LANE per region screens it from the region records the mark
-// kernel left behind and then walks just those lines; regions the records cannot settle (more than 32
-// newlines, dense neighbours, a line start further back than the previous region) take the general path.
-__global__ void __launch_bounds__(MARK_WARPS * 32) fasta_lines_kernel(const ScanParams P) {
-    const int lane = threadIdx.x & 31;
-    const int64_t R0 = ((int64_t)blockIdx.x * MARK_WARPS + (threadIdx.x >> 5)) * 32;
-    if (R0 >= P.nreg) return;
-    const int64_t r = R0 + lane;
-    const bool inb = r < P.nreg;
+// FASTA rows: one CTA per prefix block, ROWS_PER_THREAD consecutive regions per thread.  The regions' exclusive
+// counts are scanned here from rc (there is no per-region prefix array for FASTA).  Only lines that change a
+// record do any work: lines 0 and 1 of a region go through do_line (the newlines before them are the previous
+// region's last two entries, or are found by carry_walk), lines k >= 2 are the line facts mark wrote.  A general
+// region (more than 32 newlines, more than LF_MAX facts, dense) has no line facts; its exclusive counts go into its
+// fact slot instead, for fasta_general_kernel.
+constexpr int ROWS_THREADS = 1024, ROWS_PER_THREAD = PS_BLOCK / ROWS_THREADS;
+static_assert(ROWS_PER_THREAD == 4, "one uint4 of first-entry words per thread");
+
+__global__ void __launch_bounds__(ROWS_THREADS) fasta_rows_kernel(const ScanParams P) {
+    __shared__ uint32_t s_a[ROWS_THREADS / 32], s_b[ROWS_THREADS / 32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int64_t r0 = (int64_t)blockIdx.x * PS_BLOCK + (int64_t)threadIdx.x * ROWS_PER_THREAD;
+    const uint4 qa = reinterpret_cast<const uint4 *>(P.rc + r0)[0], qb = reinterpret_cast<const uint4 *>(P.rc + r0)[1];
+    const uint4 fv = *reinterpret_cast<const uint4 *>(P.fw + r0);
+    const uint2 rcv[ROWS_PER_THREAD] = {make_uint2(qa.x, qa.y), make_uint2(qa.z, qa.w), make_uint2(qb.x, qb.y), make_uint2(qb.z, qb.w)};
+    const uint32_t fwv[ROWS_PER_THREAD] = {fv.x, fv.y, fv.z, fv.w};
+    uint2 pv = r0 >= 1 ? P.rc[r0 - 1] : make_uint2(0u, 0u);
+    // exclusive {newlines, header starts} of the thread's first region
+    uint32_t a = 0, b = 0;
+#pragma unroll
+    for (int i = 0; i < ROWS_PER_THREAD; ++i) { a += rcv[i].x & 0xffffu; b += rcv[i].x >> 16; }
+    uint32_t ia = a, ib = b;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        const uint32_t oa = __shfl_up_sync(0xffffffffu, ia, d), ob = __shfl_up_sync(0xffffffffu, ib, d);
+        if (lane >= d) { ia += oa; ib += ob; }
+    }
+    const ulonglong2 bb = P.bs[blockIdx.x];
+    if (lane == 31) { s_a[warp] = ia; s_b[warp] = ib; }
+    __syncthreads();
+    uint32_t wa = 0, wb = 0;
+    for (int w = 0; w < warp; ++w) { wa += s_a[w]; wb += s_b[w]; }
+    ulonglong2 X = make_ulonglong2(bb.x + wa + ia - a, bb.y + wb + ib - b);
     unsigned long long dummy = 0;
-    uint2 me = make_uint2(0u, 0u), pv = make_uint2(0u, 0u);
-    uint4 q = make_uint4(0u, 0u, 0u, 0u);
-    ulonglong2 X = make_ulonglong2(0, 0);
-    if (inb) {
-        me = P.rc[r];
-        if (r >= 1) pv = P.rc[r - 1];
-        q = P.rec2[r];
-        X = P.ex[r];
+    bool any_general = false;
+#pragma unroll
+    for (int i = 0; i < ROWS_PER_THREAD; ++i) {
+        const int64_t r = r0 + i, base = r * REGION;
+        const uint32_t nl = rcv[i].x & 0xffffu, fw = fwv[i], pnl = pv.x & 0xffffu;
+        const bool general = nl != 0 && (fw & FW_GEN) != 0;
+        const bool walk = nl != 0 && !general && (r == 0 || pnl < 2u || pnl > (uint32_t)SEGCAP);
+        Prev2 cy;                                     // the two newlines before the region
+        cy.pos1 = base - REGION + (int64_t)(pv.y & E_POS); cy.h1 = (pv.y >> 15) & 1u;
+        cy.pos0 = base - REGION + (int64_t)((pv.y >> 16) & E_POS); cy.h0 = pv.y >> 31;
+        uint32_t wm = __ballot_sync(0xffffffffu, walk);
+        while (wm) {
+            const int f = __ffs(wm) - 1;
+            wm &= wm - 1u;
+            const Prev2 c = carry_walk<0>(P.self, shfl_i64(r, f));
+            if (lane == f) cy = c;
+        }
+        if (general) *reinterpret_cast<ulonglong2 *>(P.lf + r * LF_STRIDE) = X;
+        any_general |= general;
+        if (nl != 0 && !general) {
+            const uint32_t f0 = fw & 0xffffu, f1 = fw >> 16;
+            const int64_t p0 = base + (int64_t)(f0 & E_POS);
+            do_line<0>(P, 0, p0, cy.pos1, cy.pos0, cy.h1 != 0, cy.h0 != 0, (int64_t)X.y, (int64_t)X.x, false, dummy);
+            if (nl >= 2u)
+                do_line<0>(P, 0, base + (int64_t)(f1 & E_POS), p0, cy.pos1, (f0 & E_HDR) != 0, cy.h1 != 0,
+                           (int64_t)X.y + ((f0 & E_HDR) ? 1 : 0), (int64_t)X.x + 1, false, dummy);
+            const uint32_t nf = (fw & FW_NF) >> FW_NF_SHIFT;
+            for (uint32_t j = 0; j < nf; ++j) {
+                const uint2 lf = P.lf[r * LF_STRIDE + j];
+                const int64_t slot = (int64_t)X.y + ((lf.x >> 16) & 31u), lineidx = (int64_t)X.x + ((lf.x >> 11) & 31u);
+                if (slot >= P.tmp_cap) continue;
+                const uint32_t kind = lf.x >> 21;
+                if (kind == LF_HDR) {
+                    const int64_t p = base + (int64_t)(lf.x & E_POS), dlen = lf.y & E_POS;
+                    const int elen = 1 + (int)((lf.y >> 22) & 1u);
+                    const int64_t nlen = (lf.y & LF_CUT_UNKNOWN) ? fasta_name_len(P, p - dlen - elen, dlen) : (int64_t)((lf.y >> 11) & E_POS);
+                    fasta_header(P, slot, p, lineidx, dlen, nlen, elen);
+                } else if (kind == LF_LLEN) {
+                    P.tmp[slot].llen = lf.y;
+                } else {
+                    fasta_event(P, slot, lineidx, (int32_t)lf.y);
+                }
+            }
+        }
+        X.x += nl; X.y += rcv[i].x >> 16;
+        pv = rcv[i];
     }
-    const uint32_t nl = me.x & 0xffffu, pnl = pv.x & 0xffffu;
-    const bool full = nl != 0 && (nl > 32u || r == 0 || pnl < 2u || pnl > (uint32_t)SEGCAP || q.y == 0xffffffffu);
-    uint32_t mask = 0;
-    const uint32_t c1 = pv.y & 0xffffu, c0 = pv.y >> 16, f0 = q.x & 0xffffu, f1 = q.x >> 16;
-    if (nl != 0 && !full) {
-        const int p_c1 = (int)(c1 & E_POS) - REGION, p_c0 = (int)(c0 & E_POS) - REGION;     // relative to this region
-        const int p_f0 = (int)(f0 & E_POS), p_f1 = (int)(f1 & E_POS);
-        const int L0 = p_f0 - p_c1;
-        const bool i0 = ((c1 | c0) & E_HDR) != 0 || L0 != p_c1 - p_c0;
-        const bool i1 = nl >= 2u && (((f0 | c1) & E_HDR) != 0 || p_f1 - p_f0 != L0);
-        mask = (q.y & ~3u) | (i0 ? 1u : 0u) | (i1 ? 2u : 0u);
-        if (nl < 32u) mask &= (1u << nl) - 1u;
-    }
-    const int64_t base = r * REGION;
-    const uint16_t *sg = P.seg + r * SEGCAP;
-    while (mask) {
-        const int k = __ffs(mask) - 1;
-        mask &= mask - 1;
-        uint32_t e, m1, m2;
-        int64_t b1 = base, b2 = base;
-        if (k >= 2) { e = sg[k]; m1 = sg[k - 1]; m2 = sg[k - 2]; }
-        else if (k == 1) { e = f1; m1 = f0; m2 = c1; b2 = base - REGION; }
-        else { e = f0; m1 = c1; m2 = c0; b1 = b2 = base - REGION; }
-        do_line<0>(P, 0, base + (e & E_POS), b1 + (m1 & E_POS), b2 + (m2 & E_POS), (m1 & E_HDR) != 0, (m2 & E_HDR) != 0,
-                   (int64_t)X.y + __popc(q.z & ((1u << k) - 1u)), (int64_t)X.x + k, false, dummy);
-    }
-    uint32_t fm = __ballot_sync(0xffffffffu, full);
-    while (fm) {
-        const int f = __ffs(fm) - 1;
-        fm &= fm - 1;
-        full_region<0>(P.self, 0, R0 + f);
-    }
+    const int block_general = __syncthreads_or(any_general ? 1 : 0);
+    if (threadIdx.x == 0) P.gblk[blockIdx.x] = block_general ? 1u : 0u;
 }
 
+// FASTA general regions: one LANE per region screens the first-entries word (and loads the exclusive counts
+// fasta_rows_kernel left in the fact slot), then the warp runs its general regions one after the other.
+__global__ void __launch_bounds__(MARK_WARPS * 32) fasta_general_kernel(const ScanParams P) {
+    __shared__ ulonglong2 s_x[MARK_WARPS][32];     // the lanes' counts, so that no register holds them across the calls
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int64_t R0 = ((int64_t)blockIdx.x * MARK_WARPS + warp) * 32;
+    if (R0 >= P.nreg) return;
+    const int64_t r = R0 + lane;
+    if (!P.gblk[R0 / PS_BLOCK]) return;          // no general region in this prefix block (the usual case)
+    const bool general = r < P.nreg && (P.fw[r] & FW_GEN) != 0;   // mark flags only regions with newlines
+    if (general) s_x[warp][lane] = *reinterpret_cast<const ulonglong2 *>(P.lf + r * LF_STRIDE);
+    uint32_t gm = __ballot_sync(0xffffffffu, general);
+    while (gm) {
+        const int f = __ffs(gm) - 1;
+        gm &= gm - 1u;
+        full_region<0>(P.self, 0, R0 + f, s_x[warp][f]);
+    }
+}
 
 // ---- FASTA finalize: per-record fields from neighbouring headers + event summary ------------
 // blen  = next header start - boff (or end position)                       index.c:243,348
@@ -1018,12 +1126,25 @@ __global__ void __launch_bounds__(32) edge_kernel(const ScanParams P, int mode, 
             const int fl = __ffs(nz) - 1;
             nz &= nz - 1;
             const int64_t q = r0 + fl;
-            const int cq = (int)__shfl_sync(0xffffffffu, c, fl);
-            if (cq <= SEGCAP) {
-                for (int i = 0; i < cq && found < 3; ++i) pos[found++] = q * REGION + (int64_t)(P.seg[q * SEGCAP + i] & E_POS);
-            } else {
-                for (int64_t x = q * REGION; x < q * REGION + REGION && found < 3; ++x)
-                    if (nl_at(P, x)) pos[found++] = x;
+            // the region's bytes, 16 per lane and 512 per step (FASTA keeps no newline list for most regions)
+            for (int64_t x0 = q * REGION; x0 < q * REGION + REGION && found < 3; x0 += 512) {
+                const int64_t x = x0 + lane * 16;
+                uint32_t m = 0;                                // bit i: byte x + i is a newline
+                if (x + 16 <= P.n) {
+                    const uint4 v = *reinterpret_cast<const uint4 *>(P.file + x);
+                    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+                    for (int i = 0; i < 16; ++i) m |= (((w[i >> 2] >> (8 * (i & 3))) & 0xffu) == '\n' ? 1u : 0u) << i;
+                } else {
+                    for (int i = 0; i < 16; ++i) m |= (nl_at(P, x + i) ? 1u : 0u) << i;
+                }
+                uint32_t any = __ballot_sync(0xffffffffu, m != 0);
+                while (any && found < 3) {
+                    const int fl2 = __ffs(any) - 1;
+                    any &= any - 1u;
+                    uint32_t mm = __shfl_sync(0xffffffffu, m, fl2);
+                    while (mm && found < 3) { pos[found++] = x0 + fl2 * 16 + (__ffs(mm) - 1); mm &= mm - 1u; }
+                }
             }
         }
     }
@@ -1162,14 +1283,16 @@ static int scan_params(fxg_ctx *ctx, const fxg_file *f, int mode, int64_t base_o
     const int64_t nreg = (n + 1 + REGION - 1) / REGION;     // room for a virtual newline at n
     const int64_t nb = (nreg + PS_BLOCK - 1) / PS_BLOCK;
     const int64_t nreg_pad = nb * PS_BLOCK;
-    // tile_desc: rc[nreg_pad] | bs[nb] | ex[nreg] | rec2[nreg] (FASTA)
+    // tile_desc: rc[nreg_pad] | bs[nb] | FASTQ: ex[nreg];  FASTA: fw[nreg_pad] | gblk[nb] | lf[nreg * LF_STRIDE]
     const size_t off_bs = fxg_round_up((int64_t)nreg_pad * 8, 256);
-    const size_t off_ex = off_bs + fxg_round_up(nb * (int64_t)sizeof(ulonglong2), 256);
-    const size_t off_r2 = off_ex + fxg_round_up(nreg * (int64_t)sizeof(ulonglong2), 256);
+    const size_t off_x = off_bs + fxg_round_up(nb * (int64_t)sizeof(ulonglong2), 256);
+    const size_t off_gb = off_x + fxg_round_up(nreg_pad * (int64_t)sizeof(uint32_t), 256);
+    const size_t off_lf = off_gb + fxg_round_up(nb * (int64_t)sizeof(uint32_t), 256);
+    const size_t tile_bytes = mode == 0 ? off_lf + (size_t)nreg * LF_STRIDE * sizeof(uint2) : off_x + (size_t)nreg * sizeof(ulonglong2);
     int rc;
     if (reserve) {
         if ((rc = ctx->counters.reserve(1024))) return rc;
-        if ((rc = ctx->tile_desc.reserve(off_r2 + (mode == 0 ? (size_t)nreg * sizeof(uint4) : 0)))) return rc;
+        if ((rc = ctx->tile_desc.reserve(tile_bytes))) return rc;
         if ((rc = ctx->seg.reserve((size_t)nreg * SEGCAP * sizeof(uint16_t)))) return rc;
         const int64_t want = guess_rows(mode, n);
         if (mode == 0) {
@@ -1185,8 +1308,13 @@ static int scan_params(fxg_ctx *ctx, const fxg_file *f, int mode, int64_t base_o
     P.base_offset = base_offset; P.first_line = 0; P.flags = flags;
     P.rc = (uint2 *)ctx->tile_desc.ptr;
     P.bs = (ulonglong2 *)((uint8_t *)ctx->tile_desc.ptr + off_bs);
-    P.ex = (ulonglong2 *)((uint8_t *)ctx->tile_desc.ptr + off_ex);
-    P.rec2 = (uint4 *)((uint8_t *)ctx->tile_desc.ptr + off_r2);
+    if (mode == 0) {
+        P.fw = (uint32_t *)((uint8_t *)ctx->tile_desc.ptr + off_x);
+        P.gblk = (uint32_t *)((uint8_t *)ctx->tile_desc.ptr + off_gb);
+        P.lf = (uint2 *)((uint8_t *)ctx->tile_desc.ptr + off_lf);
+    } else {
+        P.ex = (ulonglong2 *)((uint8_t *)ctx->tile_desc.ptr + off_x);
+    }
     P.seg = (uint16_t *)ctx->seg.ptr;
     P.totals = (ScanTotals *)((uint8_t *)ctx->counters.ptr + 64);
     *tmp_slots = 0;
@@ -1228,10 +1356,11 @@ extern "C" int fxg_scan_begin(fxg_ctx *ctx, const fxg_file *f, int mode, int64_t
     }
     FXG_CUDA(cudaGetLastError());
     {
-        FxgProfScope prof(ctx, FXG_PROF_PREFIX, 4);
+        FxgProfScope prof(ctx, FXG_PROF_PREFIX, mode == 0 ? 3 : 4);
         prefix_reduce_kernel<<<(unsigned)nb, PS_THREADS, 0, ctx->stream>>>(P.rc, P.bs);
         prefix_blocks_kernel<<<1, 1024, 0, ctx->stream>>>(P.bs, nb, P.file, n, mode, P.totals);
-        prefix_expand_kernel<<<(unsigned)nb, PS_THREADS, 0, ctx->stream>>>(P.rc, P.bs, P.ex, nreg);
+        // FASTA: the rows pass scans the region counts itself (fasta_rows_kernel)
+        if (mode == 1) prefix_expand_kernel<<<(unsigned)nb, PS_THREADS, 0, ctx->stream>>>(P.rc, P.bs, P.ex, nreg);
         edge_kernel<<<1, 32, 0, ctx->stream>>>(P, mode, own_info(ctx));
     }
     FXG_CUDA(cudaGetLastError());
@@ -1254,12 +1383,13 @@ static int launch_phase_b(fxg_ctx *ctx, const ScanParams &P0, int mode, int64_t 
     FXG_CUDA(cudaMemcpyAsync(ctx->params.ptr, (uint8_t *)ctx->h_counters + 4096, sizeof(P), cudaMemcpyHostToDevice, ctx->stream));
     const int64_t nreg = P.nreg;
     {
-        FxgProfScope prof(ctx, FXG_PROF_LINES, 3);
+        FxgProfScope prof(ctx, FXG_PROF_LINES, mode == 0 ? 4 : 3);
         shard_prefix_kernel<<<1, 32, 0, ctx->stream>>>(d_all, nranks, rank, mode, P.totals);
         clear_kernel<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(P, mode, tmp_slots);
         if (mode == 0) {
-            const unsigned lgrid = (unsigned)((nreg + MARK_WARPS * 32 - 1) / (MARK_WARPS * 32));
-            fasta_lines_kernel<<<lgrid, MARK_WARPS * 32, 0, ctx->stream>>>(P);
+            const int64_t nb = (nreg + PS_BLOCK - 1) / PS_BLOCK;
+            fasta_rows_kernel<<<(unsigned)nb, ROWS_THREADS, 0, ctx->stream>>>(P);
+            fasta_general_kernel<<<(unsigned)((nreg + MARK_WARPS * 32 - 1) / (MARK_WARPS * 32)), MARK_WARPS * 32, 0, ctx->stream>>>(P);
         } else {
             const unsigned lgrid = (unsigned)((nreg + MARK_WARPS * RG - 1) / (MARK_WARPS * RG));
             fastq_records_kernel<<<lgrid, MARK_WARPS * 32, 0, ctx->stream>>>(P);
