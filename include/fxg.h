@@ -278,6 +278,29 @@ int fxg_composition_host(fxg_ctx *ctx, const fxg_file *f, const fxg_fasta_row *d
                          const int64_t *row_id, const int64_t *s, const int64_t *e, const int32_t *flags,
                          int64_t nq, int64_t *hist_host);
 
+/* ---- K8: exact pattern search on the resident file ------------------------------------------
+ * Replaces Sequence.search (src/sequence.c:519-560), which extracts the sequence and scans it with str_n_str
+ * (src/util.c:769-783), and extends it to every occurrence in a batch of queries.  The haystack of query
+ * q = (row_id[q], s[q], e[q], flags) is exactly the bytes fxg_extract_dev returns for it (FXG_X_UPPER applies); a hit
+ * is a start i with hay[i, i+m) == pattern byte for byte (case-sensitive), wholly inside [s, e); overlapping hits all
+ * count.  strands: FXG_SEARCH_PLUS matches the pattern, FXG_SEARCH_MINUS its reverse complement (the extraction
+ * complement table, case preserved) in the forward haystack; a hit reports its forward start, relative to s[q].
+ *   mode FXG_SEARCH_ALL    every hit, in (query, start, minus) order
+ *   mode FXG_SEARCH_FIRST  the first hit of each (query, strand) only, in the same order
+ * row_id == NULL: one query per row (nq == n_rows), s = 0, e = slen; s and e are then ignored.
+ * 1 <= m <= FXG_SEARCH_MAX_PATTERN; flags other than FXG_X_UPPER are FXG_EINVAL.  The result is deterministic.
+ * *out is malloc'ed (free with fxg_free_host).  Synchronises after sizing the work, after counting the hits (to size
+ * the output; FXG_SEARCH_ALL only) and at the end. */
+#define FXG_SEARCH_PIECE        4096   /* stripped bases per work item of a record with uniform lines */
+#define FXG_SEARCH_MAX_PATTERN  1024
+enum { FXG_SEARCH_PLUS = 1, FXG_SEARCH_MINUS = 2 };          /* strands mask */
+enum { FXG_SEARCH_ALL = 0, FXG_SEARCH_FIRST = 1 };            /* mode */
+typedef struct fxg_search_hit { int64_t query, start; int32_t minus, pad; } fxg_search_hit;   /* 24 B */
+int fxg_search_host(fxg_ctx *ctx, const fxg_file *f, const fxg_fasta_row *d_rows, int64_t n_rows,
+                    const int64_t *row_id, const int64_t *s, const int64_t *e, int32_t flags, int64_t nq,
+                    const uint8_t *pattern, int32_t m, int strands, int mode,
+                    fxg_search_hit **out, int64_t *n_out);
+
 /* ---- K5: batched FASTQ read fetch ----------------------------------------------------------
  * Replaces pyfastx_read_random_reader + the seq/qual getters (src/read.c:37-45,152-167,
  * 237-249): for read ids[q] copies rlen raw bytes at soff (seq) and at qoff (qual).

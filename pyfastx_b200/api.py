@@ -62,6 +62,12 @@ def reverse_complement(seq):
     return out.tobytes().decode("latin-1")
 
 
+def _search_position(start, m, minus):
+    """What Sequence.search returns for an occurrence at 0-based forward `start` of a pattern of length m: the 1-based
+    start on both strands.  (The reference returns the 1-based forward end, start + m, for '-': src/sequence.c:548-549.)"""
+    return start + 1
+
+
 def _gzip_header_len(comp):
     """bytes of the gzip member header (RFC 1952) in front of the deflate data"""
     flg = int(comp[3])
@@ -452,6 +458,22 @@ class Fasta:
             return _fast_one(a[0], a[1], a[2], a[4], i, s, e, (_cabi.X_UPPER if self.uppercase else 0) | extra).decode("latin-1")
         return self._st.engine.extract_one(self._st.dfile, self._drows, i, s, e, self._flags(extra)).decode("latin-1")
 
+    def locate(self, pattern, strand="+"):
+        """Every occurrence of `pattern` (str or bytes, compared byte for byte, case-sensitive) in every record, found by
+        the search kernel on the resident file: strand "+" the pattern, "-" its reverse complement, "both" either;
+        overlapping occurrences all count.  With uppercase=True the records are upper-cased first, as their .seq is.
+        -> (row_id int64, start int64, minus bool) arrays sorted by (row_id, start, minus); start is the 0-based start in
+        the record's forward coordinates."""
+        strands = {"+": _cabi.SEARCH_PLUS, "-": _cabi.SEARCH_MINUS, "both": _cabi.SEARCH_PLUS | _cabi.SEARCH_MINUS}.get(strand)
+        if strands is None:
+            raise ValueError('strand must be "+", "-" or "both"')
+        data = pattern.encode("latin-1") if isinstance(pattern, str) else bytes(pattern)
+        if not data or len(data) > _cabi.SEARCH_MAX_PATTERN:
+            raise ValueError("pattern length must be 1 .. %d" % _cabi.SEARCH_MAX_PATTERN)
+        self._need_index()
+        hits = self._st.engine.search(self._st.dfile, self._drows, None, None, None, self._flags(), data, strands)
+        return (hits["query"].astype(np.int64), hits["start"].astype(np.int64), hits["minus"].astype(bool))
+
     # ---- reference methods -------------------------------------------------------------------------
     def fetch(self, chrom, intervals, strand="+"):
         """1-based inclusive interval(s) of `chrom`; '-' = reverse complement of the concatenation
@@ -660,6 +682,12 @@ class Sequence:
         return self._fa._one(self._i, self._s + i, self._s + i + 1)
 
     def __contains__(self, sub):
+        if isinstance(sub, str) and 0 < len(sub) <= _cabi.SEARCH_MAX_PATTERN:
+            try:
+                data = sub.encode("latin-1")
+            except UnicodeEncodeError:
+                return False
+            return self._first_hit(data, False) is not None
         return sub in self.seq
 
     def __iter__(self):
@@ -717,11 +745,35 @@ class Sequence:
                                                     fl.ctypes.data, 1, h.ctypes.data))
         return {chr(i): int(h[0, i]) for i in range(32, 127) if h[0, i] > 0}
 
+    def _first_hit(self, data, minus):
+        """0-based start of the first occurrence of `data` (bytes, 1 .. SEARCH_MAX_PATTERN long) in this sequence, or of
+        its reverse complement if `minus`, found by the search kernel where the record lies in HBM; None if there is none"""
+        fa = self._fa
+        q = np.array([self._i, self._s, self._e], dtype=np.int64)
+        hits = fa._st.engine.search(fa._st.dfile, fa._drows, q[0:1], q[1:2], q[2:3], fa._flags(), data,
+                                    _cabi.SEARCH_MINUS if minus else _cabi.SEARCH_PLUS, first=True)
+        return int(hits["start"][0]) if hits.size else None
+
     def search(self, subseq, strand="+"):
-        """1-based position of the first match or None (reference src/sequence.c:519-560)"""
-        q = subseq if strand == "+" else reverse_complement(subseq)
+        """1-based position of the first match or None (reference src/sequence.c:519-560).  A str pattern of up to
+        SEARCH_MAX_PATTERN characters is searched on the GPU; any other pattern takes the host scan of the sequence."""
+        minus = strand != "+"
+        if isinstance(subseq, str):
+            if not subseq:
+                return 1                                       # str.find("") == 0
+            if len(subseq) <= _cabi.SEARCH_MAX_PATTERN:
+                try:
+                    data = subseq.encode("latin-1")
+                except UnicodeEncodeError:                     # the sequence holds latin-1 characters only
+                    data = None
+                if data is not None:
+                    k = self._first_hit(data, minus)
+                    return None if k is None else _search_position(k, len(data), minus)
+                if not minus:
+                    return None
+        q = reverse_complement(subseq) if minus else subseq
         k = self.seq.find(q)
-        return k + 1 if k >= 0 else None
+        return _search_position(k, len(q), minus) if k >= 0 else None
 
 
 # =================================================================================================

@@ -112,6 +112,7 @@ extern "C" void fxg_ctx_destroy(fxg_ctx *c) {
         for (int j = 0; j < 2; ++j) if (c->prof_ev[i][j]) cudaEventDestroy(c->prof_ev[i][j]);
     c->tile_desc.release(); c->seg.release(); c->row_tmp.release(); c->rows.release();
     c->counters.release(); c->params.release(); c->plan.release(); c->misc.release(); c->stage_file.release();
+    c->search.release();
     if (c->own_stream && c->stream) cudaStreamDestroy(c->stream);
     delete c;
 }

@@ -68,6 +68,7 @@ struct fxg_ctx {
     cudaEvent_t  ring_ev[32] = {};
     // scan scratch
     FxgScratch   tile_desc, seg, row_tmp, rows, counters, params, plan, misc, stage_file;
+    FxgScratch   search;                 // pattern search: per-item hit counts and offsets (fxg_search_host)
     void        *h_counters = nullptr;   // pinned, small
     void        *h_one = nullptr;        // pinned + mapped: output of single-query launches (fxg_extract_one_host)
     // single-query service (resident kernel fed through mapped host memory)
@@ -175,6 +176,25 @@ __device__ __forceinline__ uint32_t reg_const(uint32_t v) {
 }
 // byte offset (0..15) of combined-mask bit beta
 __device__ __forceinline__ int chunk_bit_to_off(int beta) { return ((7 - (beta & 7)) << 2) + (beta >> 3); }
+
+// complement LUT: comp_map (src/util.c:228-237) extended to 256 entries with identity for
+// bytes >= 128 (the reference indexes a 128-entry table out of bounds there).  Extraction's strand
+// transforms and the reverse-complement pattern of pattern search both use it.
+__device__ __forceinline__ uint8_t complement_byte(int b) {
+    const int low = (b >= 'a' && b <= 'z') ? 32 : 0;
+    const int up = b - low;
+    int r = up;
+    switch (up) {
+    case 'A': r = 'T'; break; case 'T': r = 'A'; break; case 'U': r = 'A'; break;
+    case 'C': r = 'G'; break; case 'G': r = 'C'; break;
+    case 'M': r = 'K'; break; case 'K': r = 'M'; break;
+    case 'R': r = 'Y'; break; case 'Y': r = 'R'; break;
+    case 'V': r = 'B'; break; case 'B': r = 'V'; break;
+    case 'H': r = 'D'; break; case 'D': r = 'H'; break;
+    default: break;
+    }
+    return (uint8_t)(r + low);
+}
 
 __device__ __forceinline__ uint32_t ld_volatile_u32(const uint32_t *p) {
     uint32_t v;

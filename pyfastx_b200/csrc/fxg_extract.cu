@@ -185,24 +185,6 @@ __device__ void gather_one(const uint8_t *__restrict__ file, int64_t fsize, cons
     }
 }
 
-// complement LUT: comp_map (src/util.c:228-237) extended to 256 entries with identity for
-// bytes >= 128 (the reference indexes a 128-entry table out of bounds there).
-__device__ __forceinline__ uint8_t complement_byte(int b) {
-    const int low = (b >= 'a' && b <= 'z') ? 32 : 0;
-    const int up = b - low;
-    int r = up;
-    switch (up) {
-    case 'A': r = 'T'; break; case 'T': r = 'A'; break; case 'U': r = 'A'; break;
-    case 'C': r = 'G'; break; case 'G': r = 'C'; break;
-    case 'M': r = 'K'; break; case 'K': r = 'M'; break;
-    case 'R': r = 'Y'; break; case 'Y': r = 'R'; break;
-    case 'V': r = 'B'; break; case 'B': r = 'V'; break;
-    case 'H': r = 'D'; break; case 'D': r = 'H'; break;
-    default: break;
-    }
-    return (uint8_t)(r + low);
-}
-
 // ---- fast path ("pull"): records with uniform lines ---------------------------------------------
 // Output-driven: every lane assembles one aligned 16-byte OUTPUT word per round.  The kept rank of
 // its first byte gives the source position through the slice formula (sequence.c:498-510):

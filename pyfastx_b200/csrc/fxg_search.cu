@@ -1,0 +1,436 @@
+// fxg_search.cu -- K8 exact pattern search on the resident file (sm_90a).
+//
+// Replaces Sequence.search (src/sequence.c:519-560: extract the sequence, then str_n_str, src/util.c:769-783) and
+// extends it to every occurrence in a batch of queries.  The haystack of a query is exactly what extraction returns
+// for it: the bytes are found the way serve_query_warp's strip path finds them (fxg_extract.cu), in ONE fused pass
+// over the resident file bytes -- a warp streams the covering source range, drops 10 / 13 / 32, upper-cases if asked,
+// and stages the kept bytes in its own shared-memory window, where every start position is tested against the
+// pattern and its reverse complement.  There is no stripped copy in HBM.
+//
+// Work items: a query on a record with uniform lines (norm = 1 and the scan's uniform bit) is cut into pieces of
+// FXG_SEARCH_PIECE start positions, each staged with the m - 1 bases that follow it (clipped to e) through the slice
+// formula (sequence.c:498-510), as extract_one_kernel serves the pieces of such a query.  Any other query is one item: one warp
+// streams the record from its first byte with a skip, like gather_one, matching window by window.
+//
+// Ordered output without atomics or a sort:
+//   1. items   per query, the number of items; exclusive prefix -> item offsets (host learns the item total)
+//   2. count   per item, the hits of each strand
+//   3. ALL:    exclusive prefix of the per-item hits (host learns the output size), then emit: only the items with
+//              hits run again, each writing its hits at its offset in (start, minus) order
+//      FIRST:  one warp per (query, strand) finds the first item with a hit and runs that item until its first hit
+#include "fxg_common.cuh"
+#include <stdlib.h>
+#include <string.h>
+#include <vector>
+
+namespace fxg {
+
+constexpr int SW = 8;                                       // warps per CTA
+constexpr int SPIECE = FXG_SEARCH_PIECE;
+constexpr int SMAXPAT = FXG_SEARCH_MAX_PATTERN;
+// per-warp haystack window: one piece, the m - 1 bases after it, one 512-byte gather round beyond that, and slack for
+// the word loads of the last positions
+constexpr int SHB = (SPIECE + SMAXPAT - 1 + 512 + 32 + 15) & ~15;
+constexpr int SPB = SMAXPAT + 16;                           // pattern buffers (zero padded for word compares)
+static_assert(SPIECE % 128 == 0 && SPIECE >= SMAXPAT + 512, "a window shift must not overlap itself");
+
+enum { S_COUNT = 0, S_ALL = 1, S_FIRST = 2 };
+
+struct SearchArgs {
+    const uint8_t *file;
+    int64_t fsize;
+    const fxg_fasta_row *rows;
+    int64_t n_rows;
+    const int64_t *q_row, *q_s, *q_e;       // q_row == nullptr: query q = (row q, 0, slen)
+    int64_t nq;
+    int flags, m, strands;
+    const uint8_t *pattern;
+    const int64_t *item_off;                // nq + 1
+    int64_t *tot, *pc;                      // per item: hits on both strands, hits on the plus strand
+    const int64_t *hit_off;                 // per item: first output slot (S_ALL)
+    fxg_search_hit *out;
+};
+
+__device__ __forceinline__ void load_query(const SearchArgs &A, int64_t q, int64_t &s, int64_t &e, fxg_fasta_row &r,
+                                           bool &row_ok) {
+    const int64_t rid = A.q_row ? A.q_row[q] : q;
+    row_ok = rid >= 0 && rid < A.n_rows;
+    memset(&r, 0, sizeof(r));
+    if (row_ok) r = A.rows[rid];
+    s = A.q_row ? A.q_s[q] : 0;
+    e = A.q_row ? A.q_e[q] : r.slen;
+}
+// a query that extract_one_kernel cuts into pieces
+__device__ __forceinline__ bool split_row(const fxg_fasta_row &r, bool row_ok) { return row_ok && r.norm && (r.pad[0] & 1); }
+
+// haystack bytes i .. i+3 as one little-endian word (the window is 16-byte aligned)
+__device__ __forceinline__ uint32_t word_at(const uint8_t *h, int i) {
+    const uint32_t *w = reinterpret_cast<const uint32_t *>(h) + (i >> 2);
+    return __funnelshift_r(w[0], w[1], 8 * (i & 3));
+}
+// hay[i + 4, i + m) == P[4, m): the first four bytes were compared by the caller
+__device__ __forceinline__ bool rest_equal(const uint8_t *h, int i, const uint8_t *P, int m) {
+    const uint32_t *pw = reinterpret_cast<const uint32_t *>(P);
+    for (int j = 4; j < m; j += 4) {
+        uint32_t d = word_at(h, i + j) ^ pw[j >> 2];
+        if (m - j < 4) d &= (1u << (8 * (m - j))) - 1u;
+        if (d) return false;
+    }
+    return true;
+}
+
+// Runs work item p of query q on the strands in `strands` (bit 0 plus, bit 1 minus).  S_COUNT adds the lane's hits to
+// cp / cm; S_ALL writes every hit from A.out[out_pos] on; S_FIRST writes the first hit to A.out[out_pos] and returns.
+template <int MODE>
+__device__ void run_item(const SearchArgs &A, int64_t q, int64_t p, int strands, uint8_t *__restrict__ hb,
+                         const uint8_t *__restrict__ pat, const uint8_t *__restrict__ rc, int lane, int64_t out_pos,
+                         int64_t &cp, int64_t &cm) {
+    int64_t s, e;
+    fxg_fasta_row r;
+    bool row_ok;
+    load_query(A, q, s, e, r, row_ok);
+    const int m = A.m;
+    const int64_t len = e - s;
+    int64_t a = 0, b = len, c = len;                            // starts [a, b), haystack bytes [a, c) of the query
+    if (split_row(r, row_ok)) {
+        a = p * SPIECE;
+        b = a + SPIECE < len ? a + SPIECE : len;
+        c = b + m - 1 < len ? b + m - 1 : len;
+    }
+    const int64_t ss = s + a, ee = s + c, out_len = c - a;
+    const int64_t ntest = (b - a) < (out_len - m + 1) ? (b - a) : (out_len - m + 1);
+    // the source range of [ss, ee), as serve_query_warp's strip path takes it; rows pointing outside the buffer
+    // give zero bytes, as they do there
+    int64_t src = 0, src_len = 0, skip = 0;
+    if (row_ok && r.boff >= 0 && r.blen >= 0 && r.boff <= A.fsize && ss >= 0) {
+        const int64_t bpl = r.llen - (int64_t)r.elen;
+        if (r.norm && bpl > 0 && !(ss == 0 && ee == r.slen)) {
+            const int64_t bs = ss / bpl, be = ee / bpl;                          // sequence.c:500-503
+            src = r.boff + ss + (int64_t)r.elen * bs;                            // sequence.c:508
+            src_len = (ee - ss) + (be - bs) * (int64_t)r.elen;                   // sequence.c:509
+        } else {
+            src = r.boff; src_len = r.blen; skip = ss;                           // sequence.c:100-102,108-110
+        }
+    }
+    int64_t src_end = src + src_len;
+    if (src_end > A.fsize) src_end = A.fsize;
+    const int64_t want_end = skip + out_len;
+    const bool upper = (A.flags & FXG_X_UPPER) != 0;
+    const bool want_p = (strands & 1) != 0, want_m = (strands & 2) != 0;
+    const uint32_t pmask = m >= 4 ? 0xffffffffu : (1u << (8 * m)) - 1u;
+    const uint32_t pp = *reinterpret_cast<const uint32_t *>(pat) & pmask, pm = *reinterpret_cast<const uint32_t *>(rc) & pmask;
+    const uint32_t *hw = reinterpret_cast<const uint32_t *>(hb);
+    int64_t done = 0;                                           // kept bytes seen
+    int64_t wb = 0;                                             // haystack index (from a) of hb[0]
+    int have = 0;                                               // haystack bytes in hb
+    int64_t cursor = out_pos;                                   // S_ALL: next output slot
+    for (int64_t cbase = src & ~(int64_t)15;; cbase += 512) {
+        const bool more = cbase < src_end && done < want_end;
+        if (more) {
+            const int64_t my = cbase + lane * 16;
+            uint4 v = make_uint4(0, 0, 0, 0);
+            int lo = 0, hi = 0;
+            if (my < src_end && my + 16 > src) {
+                v = *reinterpret_cast<const uint4 *>(A.file + my);
+                lo = (int)(src > my ? src - my : 0);
+                hi = (int)(src_end - my < 16 ? src_end - my : 16);
+            }
+            const uint32_t wd[4] = {v.x, v.y, v.z, v.w};
+            uint32_t keep = 0;                                  // bit j: byte j is kept
+#pragma unroll
+            for (int w = 0; w < 4; ++w) {
+                const uint32_t k = ~(byte_eq_mask(wd[w], 0x0a0a0a0au) | byte_eq_mask(wd[w], 0x0d0d0d0du) |
+                                     byte_eq_mask(wd[w], 0x20202020u)) & 0x80808080u;
+                keep |= (((k >> 7) & 1u) | ((k >> 14) & 2u) | ((k >> 21) & 4u) | ((k >> 28) & 8u)) << (4 * w);
+            }
+            keep &= ((1u << hi) - 1u) & ~((1u << lo) - 1u);
+            const int cnt = __popc(keep);
+            int incl = cnt;
+#pragma unroll
+            for (int d = 1; d < 32; d <<= 1) {
+                const int o = __shfl_up_sync(0xffffffffu, incl, d);
+                if (lane >= d) incl += o;
+            }
+            const int total = __shfl_sync(0xffffffffu, incl, 31);
+            int64_t rank = done + (incl - cnt);
+            const int64_t r0 = skip + wb;                       // kept rank of hb[0]
+            if (keep == 0xffffu && rank >= r0 && rank + 16 <= want_end) {
+                // the common case inside a line: all 16 bytes are kept and wanted, no per-byte search of the mask
+                uint8_t *d = hb + (rank - r0);
+#pragma unroll
+                for (int j = 0; j < 16; ++j) {
+                    uint32_t by = (wd[j >> 2] >> (8 * (j & 3))) & 0xffu;
+                    if (upper && by - 'a' < 26u) by -= 32;
+                    d[j] = (uint8_t)by;
+                }
+                keep = 0;
+            }
+            while (keep) {
+                const int j = __ffs(keep) - 1;
+                keep &= keep - 1;
+                if (rank >= r0 && rank < want_end) {
+                    const uint32_t wj = j < 8 ? (j < 4 ? v.x : v.y) : (j < 12 ? v.z : v.w);   // no local-memory array
+                    uint32_t by = (wj >> (8 * (j & 3))) & 0xffu;
+                    if (upper && by >= 'a' && by <= 'z') by -= 32;
+                    hb[rank - r0] = (uint8_t)by;
+                }
+                ++rank;
+            }
+            done += total;
+            __syncwarp();
+            int64_t got = done - skip;
+            got = got < 0 ? 0 : (got > out_len ? out_len : got);
+            have = (int)(got - wb);
+        }
+        while (wb < ntest) {
+            const int64_t wend = wb + SPIECE < ntest ? wb + SPIECE : ntest;
+            const int need = (int)((wend + m - 1 < out_len ? wend + m - 1 : out_len) - wb);
+            if (have < need) {
+                if (more) break;
+                // fewer kept bytes than the query asks for (malformed record): extraction defines them as 0
+                for (int i = have + lane; i < need; i += 32) hb[i] = 0;
+                __syncwarp();
+                have = need;
+            }
+            const int nt = (int)(wend - wb);
+            const int64_t start0 = a + wb;
+            for (int r0 = 0; r0 < nt; r0 += 128) {
+                const int i0 = r0 + 4 * lane;
+                const uint32_t W0 = hw[i0 >> 2], W1 = hw[(i0 >> 2) + 1];
+                uint32_t hp = 0, hm = 0;
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    const int i = i0 + k;
+                    if (i < nt) {
+                        const uint32_t w = (k ? __funnelshift_r(W0, W1, 8 * k) : W0) & pmask;
+                        if (want_p && w == pp && (m <= 4 || rest_equal(hb, i, pat, m))) hp |= 1u << k;
+                        if (want_m && w == pm && (m <= 4 || rest_equal(hb, i, rc, m))) hm |= 1u << k;
+                    }
+                }
+                if (MODE == S_COUNT) {
+                    cp += __popc(hp);
+                    cm += __popc(hm);
+                } else if (MODE == S_ALL) {
+                    const int n = __popc(hp) + __popc(hm);
+                    if (__any_sync(0xffffffffu, n != 0)) {
+                        int inc = n;
+#pragma unroll
+                        for (int d = 1; d < 32; d <<= 1) {
+                            const int o = __shfl_up_sync(0xffffffffu, inc, d);
+                            if (lane >= d) inc += o;
+                        }
+                        int64_t o = cursor + (inc - n);
+#pragma unroll
+                        for (int k = 0; k < 4; ++k) {                         // (start, minus) order
+                            if ((hp >> k) & 1u) { fxg_search_hit *h = A.out + o++; h->query = q; h->start = start0 + i0 + k; h->minus = 0; h->pad = 0; }
+                            if ((hm >> k) & 1u) { fxg_search_hit *h = A.out + o++; h->query = q; h->start = start0 + i0 + k; h->minus = 1; h->pad = 0; }
+                        }
+                        cursor += __shfl_sync(0xffffffffu, inc, 31);
+                    }
+                } else {
+                    const uint32_t h = hp | hm;                                 // one strand is asked for
+                    const uint32_t bal = __ballot_sync(0xffffffffu, h != 0);
+                    if (bal) {
+                        if (lane == __ffs(bal) - 1) {
+                            fxg_search_hit *o = A.out + out_pos;
+                            o->query = q; o->start = start0 + i0 + __ffs(h) - 1; o->minus = want_m ? 1 : 0; o->pad = 0;
+                        }
+                        return;
+                    }
+                }
+            }
+            wb = wend;
+            if (wb >= ntest) break;
+            // the next window starts PIECE bytes on: keep its first m - 1 bytes and whatever the last round brought
+            const int keepn = have - SPIECE;
+            __syncwarp();                                       // every lane is done reading the window
+            for (int i = lane; i < keepn; i += 32) hb[i] = hb[SPIECE + i];
+            __syncwarp();
+            have = keepn;
+        }
+        if (!more || wb >= ntest) break;
+    }
+}
+
+__global__ void search_items_kernel(SearchArgs A, int64_t *__restrict__ n_items) {
+    const int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= A.nq) return;
+    int64_t s, e;
+    fxg_fasta_row r;
+    bool row_ok;
+    load_query(A, q, s, e, r, row_ok);
+    const int64_t len = e - s;
+    int64_t n = 0;
+    if (len >= A.m) n = split_row(r, row_ok) ? (len - A.m + SPIECE) / SPIECE : 1;
+    n_items[q] = n;
+}
+
+template <int MODE>
+__global__ void __launch_bounds__(SW * 32, 4) search_kernel(SearchArgs A) {
+    __shared__ __align__(16) uint8_t s_pat[2][SPB];             // the pattern and its reverse complement
+    __shared__ __align__(16) uint8_t s_hay[SW][SHB];
+    const int m = A.m;
+    for (int i = threadIdx.x; i < SPB; i += blockDim.x) {
+        s_pat[0][i] = i < m ? A.pattern[i] : 0;
+        s_pat[1][i] = i < m ? complement_byte(A.pattern[m - 1 - i]) : 0;
+    }
+    __syncthreads();
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int64_t gw = (int64_t)blockIdx.x * SW + warp, nw = (int64_t)gridDim.x * SW;
+    int64_t cp = 0, cm = 0;
+    if (MODE != S_FIRST) {
+        const int64_t n_items = A.item_off[A.nq];
+        for (int64_t it = gw; it < n_items; it += nw) {
+            if (MODE == S_ALL && A.tot[it] == 0) continue;
+            int64_t lo = 0, hi = A.nq;                              // item_off[lo] <= it < item_off[hi]
+            while (hi - lo > 1) {
+                const int64_t mid = (lo + hi) >> 1;
+                if (A.item_off[mid] <= it) lo = mid; else hi = mid;
+            }
+            cp = cm = 0;
+            run_item<MODE>(A, lo, it - A.item_off[lo], A.strands, s_hay[warp], s_pat[0], s_pat[1], lane,
+                           MODE == S_ALL ? A.hit_off[it] : 0, cp, cm);
+            if (MODE == S_COUNT) {
+#pragma unroll
+                for (int d = 16; d > 0; d >>= 1) { cp += shfl_down_i64(cp, d); cm += shfl_down_i64(cm, d); }
+                if (lane == 0) { A.tot[it] = cp + cm; A.pc[it] = cp; }
+            }
+            __syncwarp();
+        }
+    } else {
+        for (int64_t w = gw; w < 2 * A.nq; w += nw) {
+            const int64_t q = w >> 1;
+            const int st = (int)(w & 1);
+            int64_t first = -1;
+            if ((A.strands >> st) & 1) {
+                const int64_t i0 = A.item_off[q], i1 = A.item_off[q + 1];
+                for (int64_t b0 = i0; b0 < i1; b0 += 32) {
+                    const int64_t it = b0 + lane;
+                    int64_t c = 0;
+                    if (it < i1) c = st ? A.tot[it] - A.pc[it] : A.pc[it];
+                    const uint32_t bal = __ballot_sync(0xffffffffu, c > 0);
+                    if (bal) { first = b0 + __ffs(bal) - 1; break; }
+                }
+            }
+            if (lane == 0) A.out[w].query = -1;
+            __syncwarp();
+            if (first >= 0)
+                run_item<S_FIRST>(A, q, first - A.item_off[q], 1 << st, s_hay[warp], s_pat[0], s_pat[1], lane, w, cp, cm);
+            __syncwarp();
+        }
+    }
+}
+
+}  // namespace fxg
+
+using namespace fxg;
+
+static int search_grid(fxg_ctx *ctx, int64_t warps) {
+    int64_t blocks = (warps + SW - 1) / SW;
+    const int64_t maxb = (int64_t)ctx->sm_count * 4;
+    if (blocks > maxb) blocks = maxb;
+    return blocks < 1 ? 1 : (int)blocks;
+}
+
+extern "C" int fxg_search_host(fxg_ctx *ctx, const fxg_file *f, const fxg_fasta_row *d_rows, int64_t n_rows,
+                               const int64_t *row_id, const int64_t *s, const int64_t *e, int32_t flags, int64_t nq,
+                               const uint8_t *pattern, int32_t m, int strands, int mode, fxg_search_hit **out,
+                               int64_t *n_out) {
+    if (!ctx && fxg_device_count() == 0) {
+        fxg_set_error("no CUDA device available; libfxg has no CPU fallback");
+        return FXG_ENODEV;
+    }
+    FXG_CHECK_ARG(ctx && f && out && n_out && pattern && nq >= 0 && n_rows >= 0, "bad arguments");
+    FXG_CHECK_ARG(m >= 1 && m <= FXG_SEARCH_MAX_PATTERN, "pattern length must be 1 .. FXG_SEARCH_MAX_PATTERN");
+    FXG_CHECK_ARG(strands >= 1 && strands <= 3, "strands must be FXG_SEARCH_PLUS, FXG_SEARCH_MINUS or both");
+    FXG_CHECK_ARG(mode == FXG_SEARCH_ALL || mode == FXG_SEARCH_FIRST, "mode must be FXG_SEARCH_ALL or FXG_SEARCH_FIRST");
+    FXG_CHECK_ARG((flags & ~FXG_X_UPPER) == 0, "flags other than FXG_X_UPPER are not searchable");
+    FXG_CHECK_ARG(row_id ? (nq == 0 || (s && e)) : nq == n_rows, "row_id, s, e: all or none (then nq == n_rows)");
+    FXG_CHECK_ARG(nq == 0 || d_rows, "d_rows == NULL");
+    *out = nullptr;
+    *n_out = 0;
+    FXG_LOCK(ctx);
+    FXG_CUDA(cudaSetDevice(ctx->device));
+    fxg_search_hit *h = nullptr;
+    int64_t n_hits = 0;
+    if (nq > 0) {
+        // misc: [row | s | e] | n_items | zeros | item_off (nq + 1) | pattern
+        const size_t qb = (size_t)nq * 8, nqa = row_id ? 3 : 0;
+        int rc = ctx->misc.reserve(qb * (nqa + 2) + qb + 8 + SPB + 64);
+        if (rc) return rc;
+        int64_t *base = (int64_t *)ctx->misc.ptr;
+        int64_t *d_row = row_id ? base : nullptr, *d_s = row_id ? base + nq : nullptr, *d_e = row_id ? base + 2 * nq : nullptr;
+        int64_t *d_nit = base + nqa * nq, *d_zero = d_nit + nq, *d_ioff = d_zero + nq;
+        uint8_t *d_pat = (uint8_t *)(d_ioff + nq + 1);
+        if (row_id) {
+            FXG_CUDA(cudaMemcpyAsync(d_row, row_id, qb, cudaMemcpyHostToDevice, ctx->stream));
+            FXG_CUDA(cudaMemcpyAsync(d_s, s, qb, cudaMemcpyHostToDevice, ctx->stream));
+            FXG_CUDA(cudaMemcpyAsync(d_e, e, qb, cudaMemcpyHostToDevice, ctx->stream));
+        }
+        FXG_CUDA(cudaMemcpyAsync(d_pat, pattern, (size_t)m, cudaMemcpyHostToDevice, ctx->stream));
+        FXG_CUDA(cudaMemsetAsync(d_zero, 0, qb, ctx->stream));
+        SearchArgs A;
+        memset(&A, 0, sizeof(A));
+        A.file = f->d; A.fsize = f->size; A.rows = d_rows; A.n_rows = n_rows;
+        A.q_row = d_row; A.q_s = d_s; A.q_e = d_e; A.nq = nq;
+        A.flags = flags; A.m = m; A.strands = strands; A.pattern = d_pat; A.item_off = d_ioff;
+        ctx->launches += 1;
+        search_items_kernel<<<(unsigned)((nq + 255) / 256), 256, 0, ctx->stream>>>(A, d_nit);
+        FXG_CUDA(cudaGetLastError());
+        int64_t n_items = 0;
+        if ((rc = fxg_extract_plan_dev(ctx, d_zero, d_nit, nq, d_ioff, &n_items))) return rc;     // synchronises
+        if (n_items > 0) {
+            // search scratch: tot | pc | zeros | hit_off (n_items + 1)
+            if ((rc = ctx->search.reserve((size_t)n_items * 32 + 8 + 64))) return rc;
+            A.tot = (int64_t *)ctx->search.ptr;
+            A.pc = A.tot + n_items;
+            int64_t *d_zero2 = A.pc + n_items, *d_hoff = d_zero2 + n_items;
+            A.hit_off = d_hoff;
+            {
+                FxgProfScope prof(ctx, FXG_PROF_GATHER);
+                search_kernel<S_COUNT><<<search_grid(ctx, n_items), SW * 32, 0, ctx->stream>>>(A);
+            }
+            FXG_CUDA(cudaGetLastError());
+            if (mode == FXG_SEARCH_ALL) {
+                FXG_CUDA(cudaMemsetAsync(d_zero2, 0, (size_t)n_items * 8, ctx->stream));
+                if ((rc = fxg_extract_plan_dev(ctx, d_zero2, A.tot, n_items, d_hoff, &n_hits))) return rc;   // synchronises
+                if (n_hits > 0) {
+                    if ((rc = ctx->row_tmp.reserve((size_t)n_hits * sizeof(fxg_search_hit) + 64))) return rc;
+                    A.out = (fxg_search_hit *)ctx->row_tmp.ptr;
+                    ctx->launches += 1;
+                    search_kernel<S_ALL><<<search_grid(ctx, n_items), SW * 32, 0, ctx->stream>>>(A);
+                    FXG_CUDA(cudaGetLastError());
+                    h = (fxg_search_hit *)malloc((size_t)n_hits * sizeof(fxg_search_hit));
+                    if (!h) { fxg_set_error("out of memory (%lld search hits)", (long long)n_hits); return FXG_ENOMEM; }
+                    cudaError_t ce = cudaMemcpyAsync(h, A.out, (size_t)n_hits * sizeof(fxg_search_hit), cudaMemcpyDeviceToHost, ctx->stream);
+                    if (ce == cudaSuccess) ce = cudaStreamSynchronize(ctx->stream);
+                    if (ce != cudaSuccess) { free(h); FXG_CUDA(ce); }
+                }
+            } else {
+                if ((rc = ctx->row_tmp.reserve((size_t)nq * 2 * sizeof(fxg_search_hit) + 64))) return rc;
+                A.out = (fxg_search_hit *)ctx->row_tmp.ptr;
+                ctx->launches += 1;
+                search_kernel<S_FIRST><<<search_grid(ctx, 2 * nq), SW * 32, 0, ctx->stream>>>(A);
+                FXG_CUDA(cudaGetLastError());
+                std::vector<fxg_search_hit> slot((size_t)nq * 2);
+                FXG_CUDA(cudaMemcpyAsync(slot.data(), A.out, slot.size() * sizeof(fxg_search_hit), cudaMemcpyDeviceToHost, ctx->stream));
+                FXG_CUDA(cudaStreamSynchronize(ctx->stream));
+                h = (fxg_search_hit *)malloc(slot.size() * sizeof(fxg_search_hit));
+                if (!h) { fxg_set_error("out of memory (%lld search hits)", (long long)nq * 2); return FXG_ENOMEM; }
+                for (int64_t q = 0; q < nq; ++q) {                   // slot 2q: plus strand, 2q + 1: minus strand
+                    const fxg_search_hit &p = slot[2 * q], &mi = slot[2 * q + 1];
+                    const bool hp = p.query >= 0, hm = mi.query >= 0;
+                    if (hp && hm && mi.start < p.start) { h[n_hits++] = mi; h[n_hits++] = p; }
+                    else { if (hp) h[n_hits++] = p; if (hm) h[n_hits++] = mi; }
+                }
+            }
+        }
+    }
+    if (!h) {
+        h = (fxg_search_hit *)malloc(sizeof(fxg_search_hit));
+        if (!h) { fxg_set_error("out of memory"); return FXG_ENOMEM; }
+    }
+    *out = h;
+    *n_out = n_hits;
+    return FXG_OK;
+}

@@ -382,6 +382,29 @@ class Engine:
         check(lib().fxg_extract_one_host(self.ctx, dfile.handle, drows.devptr, drows.n_rows, row_id, s, e, flags, buf, n))
         return buf.raw
 
+    def search(self, dfile, drows, row_id, s, e, flags, pattern, strands=_cabi.SEARCH_PLUS, first=False):
+        """Exact pattern search (K8) in the haystacks of the queries (row_id, s, e) -- the bytes extraction returns for
+        them -- or, with row_id = s = e = None, in every whole record.  -> SEARCH_HIT array of (query, start, minus) in
+        (query, start, minus) order, start relative to s; first=True keeps the first hit of each (query, strand)."""
+        pat = bytes(pattern)
+        if row_id is None:
+            nq, rp, sp, ep = drows.n_rows, None, None, None
+        else:
+            row_id = np.ascontiguousarray(row_id, dtype=np.int64)
+            s = np.ascontiguousarray(s, dtype=np.int64)
+            e = np.ascontiguousarray(e, dtype=np.int64)
+            nq, rp, sp, ep = row_id.size, ptr(row_id), ptr(s), ptr(e)
+        out = C.c_void_p()
+        n = C.c_int64(0)
+        check(lib().fxg_search_host(self.ctx, dfile.handle, drows.devptr, drows.n_rows, rp, sp, ep, int(flags), nq,
+                                    pat, len(pat), int(strands), _cabi.SEARCH_FIRST if first else _cabi.SEARCH_ALL,
+                                    C.byref(out), C.byref(n)))
+        hits = np.zeros(n.value, dtype=_cabi.SEARCH_HIT)
+        if n.value:
+            C.memmove(hits.ctypes.data, out.value, n.value * _cabi.SEARCH_HIT.itemsize)
+        lib().fxg_free_host(out)
+        return hits[["query", "start", "minus"]]
+
     def read_one(self, dfile, drows, read_id, rlen, which=0, flags=0):
         """sequence (which = 0) or quality (1) bytes of one read: one kernel launch, one synchronisation"""
         if rlen <= 0:

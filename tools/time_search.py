@@ -1,0 +1,186 @@
+#!/usr/bin/env python3
+"""Time pattern search (K8) on the GPU, after verifying what it returns.
+
+    python tools/time_search.py [--steps 10] [--warmup 2] [--records 1000000] [--big-mb 250] [--out FILE]
+
+Inputs are generated in HBM with fxg_synth_fasta_dev:
+    c2   the bench's C2 shape: 1 M FASTA records of U[9000, 11000] bp at 80 columns (~10.2 GB)
+    big  one record of --big-mb million bases at 80 columns
+
+Timed (CUDA events on the search's stream around `steps` consecutive calls, each of which ends in a host
+synchronisation, divided by `steps`):
+    locate    every occurrence in every C2 record (what Fasta.locate runs) of a rare 12-mer and of GAATTC, on "+" and on
+              "both"; GB/s is file bytes over call time, and its fraction of the H100 SXM's 3.35 TB/s data-sheet figure
+    search    Sequence.search's call (first hit of one query) on the big record, against the path it replaces: extract
+              the record to the host, decode it, str.find
+
+Before any time is printed: every reported C2 hit's window, extracted with fxg_extract_host, equals the pattern (or its
+reverse complement on the minus strand), and the per-record hit counts of the first 20,000 records equal those found in
+the oracle's haystacks of the same bytes.  The GPU's name, power limit and maximum SM clock are printed with the numbers.
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+HBM_TBS = 3.35
+RARE = b"ACGTTGCATGCA"
+ECORI = b"GAATTC"
+N_ORACLE = 20000
+
+
+def gpu_info():
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
+        name, power, clock = [x.strip() for x in q.split(",")]
+        return {"name": name, "power_limit": power, "max_sm_clock": clock}
+    except Exception as ex:                                     # reported, never guessed
+        return {"error": str(ex)}
+
+
+def make_fasta(eng, lengths, width=80, seed=20240601):
+    from pyfastx_b200 import _cabi, synth
+    n = lengths.size
+    off = np.zeros(n + 1, dtype=np.int64)
+    np.cumsum(synth.fasta_record_sizes(lengths, width=width), out=off[1:])
+    f = eng.alloc_file(int(off[-1]))
+    dl, do = eng.upload_rows(lengths), eng.upload_rows(off)
+    _cabi.check(_cabi.lib().fxg_synth_fasta_dev(eng.ctx, seed, dl.devptr, do.devptr, n, 0, width, f.devptr))
+    eng.sync()
+    dl.free(); do.free()
+    return f, off
+
+
+def timed(stream, steps, fn):
+    import torch
+    ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    ev0.record(stream)
+    for _ in range(steps):
+        fn()
+    ev1.record(stream)
+    ev1.synchronize()
+    return ev0.elapsed_time(ev1) / steps
+
+
+def verify_c2(eng, f, off, drows, rows, pat, hits):
+    """hit windows through the extraction kernel; per-record counts of the first records against the oracle"""
+    from oracle import fxo
+    from pyfastx_b200 import _cabi
+    lut = fxo.complement_lut()
+    rc = bytes(lut[np.frombuffer(pat, np.uint8)][::-1])
+    m = len(pat)
+    q, st, mi = hits["query"], hits["start"], hits["minus"].astype(bool)
+    if q.size:
+        out, _, _ = eng.extract(f, drows, q, st, st + m, np.zeros(q.size, np.int32))
+        win = out.reshape(-1, m)
+        want = np.where(mi[:, None], np.frombuffer(rc, np.uint8)[None, :], np.frombuffer(pat, np.uint8)[None, :])
+        assert np.array_equal(win, want), "a reported hit's window differs from the pattern"
+    n = min(N_ORACLE, len(rows))
+    head = f.download(0, int(off[n]))
+    orows, _, _ = fxo.fasta_scan(head)
+    assert len(orows) == n
+    hay, hoff, _ = fxo.subseq_batch(head, orows, np.arange(n), np.zeros(n, np.int64), orows["slen"], np.zeros(n, np.int32))
+    hb = hay.tobytes()
+    exp = np.zeros((n, 2), dtype=np.int64)
+    for i in range(n):
+        h = hb[hoff[i]:hoff[i + 1]]
+        for s, p in ((0, pat), (1, rc)):
+            k = h.find(p)
+            while k >= 0:
+                exp[i, s] += 1
+                k = h.find(p, k + 1)
+    sel = q < n
+    got = np.zeros((n, 2), dtype=np.int64)
+    np.add.at(got, (q[sel], mi[sel].astype(np.int64)), 1)
+    assert np.array_equal(got, exp), "hit counts of the first records differ from the oracle"
+    return int(exp.sum())
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=10)
+    ap.add_argument("--warmup", type=int, default=2)
+    ap.add_argument("--records", type=int, default=1000000)
+    ap.add_argument("--big-mb", type=int, default=250)
+    ap.add_argument("--out", default=None)
+    a = ap.parse_args()
+    import torch
+    from pyfastx_b200 import _cabi, engine, synth
+    torch.cuda.init()
+    eng = engine.Engine(0)
+    stream = torch.cuda.Stream()
+    eng.set_stream(stream.cuda_stream)
+    res = {"gpu": gpu_info(), "device": torch.cuda.get_device_name(0), "locate": {}, "search": {}}
+
+    lengths = synth.fasta_lengths(a.records, 20240601, 9000, 11000)
+    f, off = make_fasta(eng, lengths)
+    rows, st, drows = eng.fasta_scan(f, keep_device_rows=True)
+    assert len(rows) == a.records
+    res["c2"] = {"file_gb": f.size / 1e9, "records": len(rows), "bases": int(st["total_len"])}
+    both = _cabi.SEARCH_PLUS | _cabi.SEARCH_MINUS
+    for name, pat in (("rare_12mer", RARE), ("GAATTC", ECORI)):
+        hits = eng.search(f, drows, None, None, None, 0, pat, both)
+        checked = verify_c2(eng, f, off, drows, rows, pat, hits)
+        for strand, mask in (("+", _cabi.SEARCH_PLUS), ("both", both)):
+            call = lambda: eng.search(f, drows, None, None, None, 0, pat, mask)
+            for _ in range(a.warmup):
+                call()
+            n_hits = len(call())
+            ms = [timed(stream, a.steps, call) for _ in range(3)]
+            med = float(np.median(ms))
+            gbs = f.size / (med * 1e-3) / 1e9
+            res["locate"]["%s %s" % (name, strand)] = {
+                "hits": n_hits, "ms_median": round(med, 3), "ms_min": round(min(ms), 3), "ms_max": round(max(ms), 3),
+                "file_GBps": round(gbs, 1), "fraction_of_3.35TBps": round(gbs / 1e3 / HBM_TBS, 3),
+                "oracle_checked_hits_first_%d_records" % N_ORACLE: checked}
+    drows.free(); f.free()
+
+    big = np.array([a.big_mb * 1000000], dtype=np.int64)
+    f, off = make_fasta(eng, big, seed=7)
+    rows, _, drows = eng.fasta_scan(f, keep_device_rows=True)
+    slen = int(rows["slen"][0])
+    rid, s0, e0 = np.array([0]), np.array([0]), np.array([slen])
+    seq_tail = eng.extract(f, drows, rid, e0 - 40, e0, np.zeros(1, np.int32))[0].tobytes()
+    for name, pat in (("rare_12mer", RARE), ("near_end_20mer", seq_tail[5:25])):
+        def gpu_first(strands=_cabi.SEARCH_PLUS):
+            h = eng.search(f, drows, rid, s0, e0, 0, pat, strands, first=True)
+            return int(h["start"][0]) + 1 if h.size else None
+        def host_find():
+            k = eng.extract_one(f, drows, 0, 0, slen, 0).decode("latin-1").find(pat.decode())
+            return k + 1 if k >= 0 else None
+        g, hst = gpu_first(), host_find()
+        assert g == hst, (name, g, hst)
+        for _ in range(a.warmup):
+            gpu_first()
+        tg = []
+        for _ in range(3):
+            t0 = time.perf_counter()
+            for _ in range(a.steps):
+                gpu_first()
+            tg.append((time.perf_counter() - t0) / a.steps * 1e3)
+        th = []
+        for _ in range(3):
+            t0 = time.perf_counter()
+            host_find()
+            th.append((time.perf_counter() - t0) * 1e3)
+        res["search"][name] = {"record_bases": slen, "answer": g, "gpu_ms_median": round(float(np.median(tg)), 3),
+                               "extract_decode_find_ms_median": round(float(np.median(th)), 1),
+                               "speedup": round(float(np.median(th)) / float(np.median(tg)), 1)}
+    drows.free(); f.free()
+    s = json.dumps(res, indent=1)
+    if a.out:
+        with open(a.out, "w") as fh:
+            fh.write(s + "\n")
+    print(s)
+
+
+if __name__ == "__main__":
+    main()
