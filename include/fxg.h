@@ -300,6 +300,18 @@ int fxg_search_host(fxg_ctx *ctx, const fxg_file *f, const fxg_fasta_row *d_rows
                     const int64_t *row_id, const int64_t *s, const int64_t *e, int32_t flags, int64_t nq,
                     const uint8_t *pattern, int32_t m, int strands, int mode,
                     fxg_search_hit **out, int64_t *n_out);
+/* K8 on FASTQ reads: every occurrence of the pattern in every read of d_rows (the complete reads of a scan or of a
+ * loaded .fxi).  The haystack of read i is exactly Read.seq (src/read.c:152-167): the rlen raw bytes at soff, nothing
+ * stripped or upper-cased ('\r' is already outside rlen), so a space inside a sequence line is part of the read and a
+ * match never runs into the line end, the '+' line, the quality line or the next read.  A hit is a start k with
+ * hay[k, k+m) == pattern byte for byte (case-sensitive); overlapping hits all count; strands as for fxg_search_host.
+ * query = the read's 0-based row index, start = the forward 0-based start.  Every hit, in (query, start, minus) order;
+ * the result is deterministic.  A row whose [soff, soff + rlen) is not inside the buffer has no hits.  Reads longer
+ * than FXG_SEARCH_PIECE bases are searched in pieces of FXG_SEARCH_PIECE start positions, shorter ones 32 at a time.
+ * 1 <= m <= FXG_SEARCH_MAX_PATTERN; n_rows == 0 gives no hits.  *out is malloc'ed (free with fxg_free_host).
+ * Synchronises after sizing the work, after counting the hits and at the end. */
+int fxg_search_reads_host(fxg_ctx *ctx, const fxg_file *f, const fxg_fastq_row *d_rows, int64_t n_rows,
+                          const uint8_t *pattern, int32_t m, int strands, fxg_search_hit **out, int64_t *n_out);
 
 /* ---- K5: batched FASTQ read fetch ----------------------------------------------------------
  * Replaces pyfastx_read_random_reader + the seq/qual getters (src/read.c:37-45,152-167,

@@ -127,6 +127,7 @@ SIGNATURES = {
     "fxg_extract_one_host": (i32, [vp, vp, vp, i64, i64, i64, i64, i32, vp, i64]),
     "fxg_composition_host": (i32, [vp, vp, vp, i64, vp, vp, vp, vp, i64, vp]),
     "fxg_search_host": (i32, [vp, vp, vp, i64, vp, vp, vp, i32, i64, vp, i32, i32, i32, P(vp), P(i64)]),
+    "fxg_search_reads_host": (i32, [vp, vp, vp, i64, vp, i32, i32, P(vp), P(i64)]),
     "fxg_reads_dev": (i32, [vp, vp, vp, i64, vp, i64, i32, vp, vp, vp, i64, P(i64)]),
     "fxg_reads_host": (i32, [vp, vp, vp, i64, vp, i64, i32, vp, vp, vp, i64]),
     "fxg_read_one_host": (i32, [vp, vp, vp, i64, i64, i32, i32, i64, vp, i64]),

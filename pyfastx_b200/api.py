@@ -68,6 +68,21 @@ def _search_position(start, m, minus):
     return start + 1
 
 
+def _locate_args(pattern, strand):
+    """(pattern bytes, strands mask) of a locate call; ValueError for a bad strand or pattern length"""
+    strands = {"+": _cabi.SEARCH_PLUS, "-": _cabi.SEARCH_MINUS, "both": _cabi.SEARCH_PLUS | _cabi.SEARCH_MINUS}.get(strand)
+    if strands is None:
+        raise ValueError('strand must be "+", "-" or "both"')
+    data = pattern.encode("latin-1") if isinstance(pattern, str) else bytes(pattern)
+    if not data or len(data) > _cabi.SEARCH_MAX_PATTERN:
+        raise ValueError("pattern length must be 1 .. %d" % _cabi.SEARCH_MAX_PATTERN)
+    return data, strands
+
+
+def _locate_result(hits):
+    return (hits["query"].astype(np.int64), hits["start"].astype(np.int64), hits["minus"].astype(bool))
+
+
 def _gzip_header_len(comp):
     """bytes of the gzip member header (RFC 1952) in front of the deflate data"""
     flg = int(comp[3])
@@ -464,15 +479,10 @@ class Fasta:
         overlapping occurrences all count.  With uppercase=True the records are upper-cased first, as their .seq is.
         -> (row_id int64, start int64, minus bool) arrays sorted by (row_id, start, minus); start is the 0-based start in
         the record's forward coordinates."""
-        strands = {"+": _cabi.SEARCH_PLUS, "-": _cabi.SEARCH_MINUS, "both": _cabi.SEARCH_PLUS | _cabi.SEARCH_MINUS}.get(strand)
-        if strands is None:
-            raise ValueError('strand must be "+", "-" or "both"')
-        data = pattern.encode("latin-1") if isinstance(pattern, str) else bytes(pattern)
-        if not data or len(data) > _cabi.SEARCH_MAX_PATTERN:
-            raise ValueError("pattern length must be 1 .. %d" % _cabi.SEARCH_MAX_PATTERN)
+        data, strands = _locate_args(pattern, strand)
         self._need_index()
-        hits = self._st.engine.search(self._st.dfile, self._drows, None, None, None, self._flags(), data, strands)
-        return (hits["query"].astype(np.int64), hits["start"].astype(np.int64), hits["minus"].astype(bool))
+        return _locate_result(self._st.engine.search(self._st.dfile, self._drows, None, None, None, self._flags(), data,
+                                                     strands))
 
     # ---- reference methods -------------------------------------------------------------------------
     def fetch(self, chrom, intervals, strand="+"):
@@ -879,6 +889,16 @@ class Fastq:
         flags = _RC if strand_minus else 0
         return self._st.engine.reads(self._st.dfile, self._drows, ids, flags=flags, want_qual=want_qual,
                                      rlens=self._rows["rlen"][ids])
+
+    def locate(self, pattern, strand="+"):
+        """Every occurrence of `pattern` (str or bytes, compared byte for byte, case-sensitive) in every read's sequence
+        (exactly Read.seq: nothing stripped or upper-cased), found by the search kernel on the resident file: strand "+"
+        the pattern, "-" its reverse complement, "both" either; overlapping occurrences all count, and no occurrence runs
+        past the end of its read.  -> (read_id int64, start int64, minus bool) arrays sorted by (read_id, start, minus);
+        fq[int(read_id[k])] is the read of hit k, start its 0-based forward start."""
+        data, strands = _locate_args(pattern, strand)
+        self.build_index()
+        return _locate_result(self._st.engine.search_reads(self._st.dfile, self._drows, data, strands))
 
     def _calc_composition(self):
         """pyfastx_fastq_calc_composition (src/fastq.c:663-795): base totals, min / max length and quality, phred

@@ -321,6 +321,223 @@ __global__ void __launch_bounds__(SW * 32, 4) search_kernel(SearchArgs A) {
     }
 }
 
+// ---- K8 on FASTQ reads ----------------------------------------------------------------------------------------------
+// The haystack of read i is its raw rlen bytes at soff (Read.seq, src/read.c:152-167).  Work items, in read order: a
+// tile is 32 consecutive read ids; each run of short reads (rlen <= SPIECE) between the tile's long reads is one item,
+// and each long read adds one item per SPIECE start positions (a piece: those starts and the m - 1 bytes after them, one
+// contiguous byte range, since a read is one line).  An item is up to 32 segments, one per lane: the lane's read, or the
+// lane's piece.  A round stages as many whole segments as the warp's window holds, each in its own slot of aligned
+// 16-byte chunks (every cp.async of the round is issued before any is consumed), then every lane tests the 16 starts of
+// one chunk.  A start is tested only below its segment's npos, so no match runs past the end of its read.
+constexpr int RW = 4;                                       // warps per CTA
+constexpr int RWIN = 8192;                                  // staging window per warp
+constexpr int RCH = RWIN / 16;                              // ... in 16-byte chunks
+static_assert(RCH >= (15 + SPIECE + SMAXPAT - 1 + 15) / 16, "a piece must fit the window in one round");
+
+struct ReadSearchArgs {
+    const uint8_t *file;
+    int64_t fsize;
+    const fxg_fastq_row *rows;
+    int64_t n_rows, n_tiles;
+    int m, strands;
+    const uint8_t *pattern;
+    const int64_t *tile_off;                // n_tiles + 1: first item of each tile
+    int64_t *tot;                           // per item: hits on both strands
+    const int64_t *hit_off;                 // per item: first output slot (S_ALL)
+    fxg_search_hit *out;
+};
+
+__device__ __forceinline__ void cp_async16(void *smem_dst, const void *gsrc) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem_dst)), "l"(gsrc) : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+
+// Lane's read of tile t: its haystack [soff, soff + len) (len = 0 for a row outside the buffer), whether it is long,
+// and how many items it starts.  brk: lanes that end a run of short reads (long reads and lanes past the last row).
+__device__ __forceinline__ int64_t tile_items(const ReadSearchArgs &A, int64_t t, int lane, int64_t &soff, int64_t &len,
+                                              uint32_t &brk) {
+    const int64_t r = t * 32 + lane;
+    const bool valid = r < A.n_rows;
+    soff = 0;
+    len = 0;
+    if (valid) {
+        const fxg_fastq_row row = A.rows[r];
+        if (row.soff >= 0 && row.rlen >= 0 && row.soff <= A.fsize && row.rlen <= A.fsize - row.soff) {
+            soff = row.soff;
+            len = row.rlen;
+        }
+    }
+    const bool lng = len > SPIECE;
+    brk = __ballot_sync(0xffffffffu, lng || !valid);
+    if (lng) return (len - A.m + SPIECE) / SPIECE;
+    return valid && (lane == 0 || ((brk >> (lane - 1)) & 1u)) ? 1 : 0;
+}
+
+__global__ void search_reads_plan_kernel(ReadSearchArgs A, int64_t *__restrict__ n_items) {
+    const int64_t t = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (t >= A.n_tiles) return;                                 // warp-uniform
+    int64_t soff, len;
+    uint32_t brk;
+    int64_t n = tile_items(A, t, threadIdx.x & 31, soff, len, brk);
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) n += shfl_down_i64(n, d);
+    if ((threadIdx.x & 31) == 0) n_items[t] = n;
+}
+
+// Every warp runs a contiguous range of items.  S_COUNT writes each item's hits to A.tot; S_ALL re-runs the items with
+// hits and writes them from A.hit_off[item] on, in (read, start, minus) order.
+template <int MODE>
+__global__ void __launch_bounds__(RW * 32) search_reads_kernel(ReadSearchArgs A) {
+    __shared__ __align__(16) uint8_t s_pat[2][SPB];
+    __shared__ __align__(16) uint8_t s_win[RW][RWIN + 16];      // + one word read past the last chunk
+    __shared__ uint8_t s_map[RW][RCH];                           // chunk -> lane whose segment it holds
+    const int m = A.m;
+    for (int i = threadIdx.x; i < SPB; i += blockDim.x) {
+        s_pat[0][i] = i < m ? A.pattern[i] : 0;
+        s_pat[1][i] = i < m ? complement_byte(A.pattern[m - 1 - i]) : 0;
+    }
+    __syncthreads();
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    uint8_t *win = s_win[warp], *map = s_map[warp];
+    const uint32_t *hw = reinterpret_cast<const uint32_t *>(win);
+    const bool want_p = (A.strands & 1) != 0, want_m = (A.strands & 2) != 0;
+    const uint32_t pmask = m >= 4 ? 0xffffffffu : (1u << (8 * m)) - 1u;
+    const uint32_t pp = *reinterpret_cast<const uint32_t *>(s_pat[0]) & pmask;
+    const uint32_t pm = *reinterpret_cast<const uint32_t *>(s_pat[1]) & pmask;
+
+    const int64_t n_items = A.tile_off[A.n_tiles];
+    const int64_t nw = (int64_t)gridDim.x * RW, per = (n_items + nw - 1) / nw;
+    int64_t it = ((int64_t)blockIdx.x * RW + warp) * per;
+    const int64_t it_end = it + per < n_items ? it + per : n_items;
+    if (it >= it_end) return;
+    int64_t t = 0, hi = A.n_tiles;                              // tile_off[t] <= it < tile_off[hi]
+    while (hi - t > 1) {
+        const int64_t mid = (t + hi) >> 1;
+        if (A.tile_off[mid] <= it) t = mid; else hi = mid;
+    }
+    int64_t loaded = -1, soff = 0, len = 0, items = 0, excl = 0;
+    uint32_t brk = 0;
+    for (; it < it_end; ++it) {
+        if (MODE == S_ALL && A.tot[it] == 0) continue;
+        while (A.tile_off[t + 1] <= it) ++t;
+        if (t != loaded) {                                      // lane j holds read 32 t + j: one coalesced 1 KiB load
+            loaded = t;
+            items = tile_items(A, t, lane, soff, len, brk);
+            int64_t inc = items;
+#pragma unroll
+            for (int d = 1; d < 32; d <<= 1) {
+                const int64_t o = shfl_up_i64(inc, d);
+                if (lane >= d) inc += o;
+            }
+            excl = inc - items;
+        }
+        // the item: lanes [js, je) -- one long read's piece, or a run of short reads
+        const int64_t li = it - A.tile_off[t];
+        const int js = __ffs(__ballot_sync(0xffffffffu, excl + items > li)) - 1;
+        const bool slong = __shfl_sync(0xffffffffu, (int)(len > SPIECE), js) != 0;
+        const uint32_t above = brk & ~((2u << js) - 1u);
+        const int je = slong ? js + 1 : (above ? __ffs(above) - 1 : 32);
+        int64_t a = 0, npos = 0;                                // segment: starts [a, a + npos) of the read
+        if (lane >= js && lane < je) {
+            if (slong) {
+                a = (li - excl) * SPIECE;
+                npos = len - m + 1 - a < SPIECE ? len - m + 1 - a : SPIECE;
+            } else {
+                npos = len - m + 1 > 0 ? len - m + 1 : 0;
+            }
+        }
+        const int64_t so = soff + a;
+        const int lead = (int)(so & 15), np = (int)npos;
+        const int nch = npos > 0 ? (lead + (int)(npos + m - 1) + 15) >> 4 : 0;
+        const int64_t gch = so >> 4;                            // first source chunk of the segment
+        int64_t cnt = 0, cursor = MODE == S_ALL ? A.hit_off[it] : 0;
+        for (int first = 0;;) {
+            // this round: the segments of lanes first .. last whose chunks fit the window
+            const int c = lane >= first ? nch : 0;
+            int incl = c;
+#pragma unroll
+            for (int d = 1; d < 32; d <<= 1) {
+                const int o = __shfl_up_sync(0xffffffffu, incl, d);
+                if (lane >= d) incl += o;
+            }
+            const bool take = lane >= first && incl <= RCH;
+            const uint32_t rest = __ballot_sync(0xffffffffu, lane >= first && !take);
+            const int C = __shfl_sync(0xffffffffu, incl, rest ? __ffs(rest) - 2 : 31);
+            const int P = incl - c;                             // slot of the lane's segment, in chunks
+            __syncwarp();                                       // every lane is done with the last round's window
+            if (take)
+                for (int k = 0; k < c; ++k) map[P + k] = (uint8_t)lane;
+            __syncwarp();
+            for (int b = 0; b < C; b += 32) {
+                const int i = b + lane;
+                const int j = i < C ? map[i] : 0;
+                const int64_t g = shfl_i64(gch, j);
+                const int pj = __shfl_sync(0xffffffffu, P, j);
+                if (i < C) cp_async16(win + 16 * i, A.file + ((g + (i - pj)) << 4));
+            }
+            cp_async_wait_all();
+            __syncwarp();
+            for (int b = 0; b < C; b += 32) {
+                const int ci = b + lane;
+                const int j = ci < C ? map[ci] : 0;
+                const int pj = __shfl_sync(0xffffffffu, P, j), lj = __shfl_sync(0xffffffffu, lead, j);
+                const int nj = __shfl_sync(0xffffffffu, np, j);
+                const int k0 = 16 * (ci - pj) - lj;             // segment start of the chunk's byte 0
+                const int lo = k0 < 0 ? -k0 : 0, hi2 = nj - k0 < 16 ? nj - k0 : 16;
+                const uint32_t valid = ci < C && hi2 > lo ? (0xffffu >> (16 - hi2)) & ~((1u << lo) - 1u) : 0u;
+                uint32_t hp = 0, hm = 0;
+                if (valid) {
+                    const uint4 v = *reinterpret_cast<const uint4 *>(win + 16 * ci);
+                    const uint32_t W[5] = {v.x, v.y, v.z, v.w, hw[4 * ci + 4]};
+#pragma unroll
+                    for (int q = 0; q < 16; ++q) {
+                        const uint32_t w = ((q & 3) ? __funnelshift_r(W[q >> 2], W[(q >> 2) + 1], 8 * (q & 3)) : W[q >> 2]) & pmask;
+                        hp |= (uint32_t)(want_p && w == pp) << q;
+                        hm |= (uint32_t)(want_m && w == pm) << q;
+                    }
+                    hp &= valid;
+                    hm &= valid;
+                    if (m > 4) {
+                        for (uint32_t x = hp; x; x &= x - 1u)
+                            if (!rest_equal(win, 16 * ci + __ffs(x) - 1, s_pat[0], m)) hp &= ~(x & (0u - x));
+                        for (uint32_t x = hm; x; x &= x - 1u)
+                            if (!rest_equal(win, 16 * ci + __ffs(x) - 1, s_pat[1], m)) hm &= ~(x & (0u - x));
+                    }
+                }
+                if (MODE == S_COUNT) {
+                    cnt += __popc(hp) + __popc(hm);
+                } else {
+                    const int64_t aj = shfl_i64(a, j);
+                    const int n = __popc(hp) + __popc(hm);
+                    if (__any_sync(0xffffffffu, n != 0)) {
+                        int inc = n;
+#pragma unroll
+                        for (int d = 1; d < 32; d <<= 1) {
+                            const int o = __shfl_up_sync(0xffffffffu, inc, d);
+                            if (lane >= d) inc += o;
+                        }
+                        int64_t o = cursor + (inc - n);
+                        const int64_t rid = t * 32 + j, s0 = aj + k0;
+                        for (uint32_t x = hp | hm; x; x &= x - 1u) {                // (start, minus) order
+                            const int q = __ffs(x) - 1;
+                            if ((hp >> q) & 1u) { fxg_search_hit *h = A.out + o++; h->query = rid; h->start = s0 + q; h->minus = 0; h->pad = 0; }
+                            if ((hm >> q) & 1u) { fxg_search_hit *h = A.out + o++; h->query = rid; h->start = s0 + q; h->minus = 1; h->pad = 0; }
+                        }
+                        cursor += __shfl_sync(0xffffffffu, inc, 31);
+                    }
+                }
+            }
+            if (!rest) break;
+            first = __ffs(rest) - 1;
+        }
+        if (MODE == S_COUNT) {
+#pragma unroll
+            for (int d = 16; d > 0; d >>= 1) cnt += shfl_down_i64(cnt, d);
+            if (lane == 0) A.tot[it] = cnt;
+        }
+    }
+}
+
 }  // namespace fxg
 
 using namespace fxg;
@@ -330,6 +547,29 @@ static int search_grid(fxg_ctx *ctx, int64_t warps) {
     const int64_t maxb = (int64_t)ctx->sm_count * 4;
     if (blocks > maxb) blocks = maxb;
     return blocks < 1 ? 1 : (int)blocks;
+}
+
+// Every hit of a count pass: the exclusive prefix of the per-item hits d_tot sizes the output (synchronises), emit(out)
+// launches the pass that writes it on the device, one D2H copy brings it back.  d_zero and d_hoff: n_items and
+// n_items + 1 scratch entries.
+template <class Emit>
+static int collect_hits(fxg_ctx *ctx, int64_t n_items, const int64_t *d_tot, int64_t *d_zero, int64_t *d_hoff, Emit emit,
+                        fxg_search_hit **h, int64_t *n_hits) {
+    FXG_CUDA(cudaMemsetAsync(d_zero, 0, (size_t)n_items * 8, ctx->stream));
+    int rc = fxg_extract_plan_dev(ctx, d_zero, d_tot, n_items, d_hoff, n_hits);
+    if (rc || *n_hits == 0) return rc;
+    if ((rc = ctx->row_tmp.reserve((size_t)*n_hits * sizeof(fxg_search_hit) + 64))) return rc;
+    fxg_search_hit *d_out = (fxg_search_hit *)ctx->row_tmp.ptr;
+    ctx->launches += 1;
+    emit(d_out);
+    FXG_CUDA(cudaGetLastError());
+    fxg_search_hit *p = (fxg_search_hit *)malloc((size_t)*n_hits * sizeof(fxg_search_hit));
+    if (!p) { fxg_set_error("out of memory (%lld search hits)", (long long)*n_hits); return FXG_ENOMEM; }
+    cudaError_t ce = cudaMemcpyAsync(p, d_out, (size_t)*n_hits * sizeof(fxg_search_hit), cudaMemcpyDeviceToHost, ctx->stream);
+    if (ce == cudaSuccess) ce = cudaStreamSynchronize(ctx->stream);
+    if (ce != cudaSuccess) { free(p); FXG_CUDA(ce); }
+    *h = p;
+    return FXG_OK;
 }
 
 extern "C" int fxg_search_host(fxg_ctx *ctx, const fxg_file *f, const fxg_fasta_row *d_rows, int64_t n_rows,
@@ -392,20 +632,11 @@ extern "C" int fxg_search_host(fxg_ctx *ctx, const fxg_file *f, const fxg_fasta_
             }
             FXG_CUDA(cudaGetLastError());
             if (mode == FXG_SEARCH_ALL) {
-                FXG_CUDA(cudaMemsetAsync(d_zero2, 0, (size_t)n_items * 8, ctx->stream));
-                if ((rc = fxg_extract_plan_dev(ctx, d_zero2, A.tot, n_items, d_hoff, &n_hits))) return rc;   // synchronises
-                if (n_hits > 0) {
-                    if ((rc = ctx->row_tmp.reserve((size_t)n_hits * sizeof(fxg_search_hit) + 64))) return rc;
-                    A.out = (fxg_search_hit *)ctx->row_tmp.ptr;
-                    ctx->launches += 1;
+                rc = collect_hits(ctx, n_items, A.tot, d_zero2, d_hoff, [&](fxg_search_hit *o) {
+                    A.out = o;
                     search_kernel<S_ALL><<<search_grid(ctx, n_items), SW * 32, 0, ctx->stream>>>(A);
-                    FXG_CUDA(cudaGetLastError());
-                    h = (fxg_search_hit *)malloc((size_t)n_hits * sizeof(fxg_search_hit));
-                    if (!h) { fxg_set_error("out of memory (%lld search hits)", (long long)n_hits); return FXG_ENOMEM; }
-                    cudaError_t ce = cudaMemcpyAsync(h, A.out, (size_t)n_hits * sizeof(fxg_search_hit), cudaMemcpyDeviceToHost, ctx->stream);
-                    if (ce == cudaSuccess) ce = cudaStreamSynchronize(ctx->stream);
-                    if (ce != cudaSuccess) { free(h); FXG_CUDA(ce); }
-                }
+                }, &h, &n_hits);
+                if (rc) return rc;
             } else {
                 if ((rc = ctx->row_tmp.reserve((size_t)nq * 2 * sizeof(fxg_search_hit) + 64))) return rc;
                 A.out = (fxg_search_hit *)ctx->row_tmp.ptr;
@@ -425,6 +656,85 @@ extern "C" int fxg_search_host(fxg_ctx *ctx, const fxg_file *f, const fxg_fasta_
                 }
             }
         }
+    }
+    if (!h) {
+        h = (fxg_search_hit *)malloc(sizeof(fxg_search_hit));
+        if (!h) { fxg_set_error("out of memory"); return FXG_ENOMEM; }
+    }
+    *out = h;
+    *n_out = n_hits;
+    return FXG_OK;
+}
+
+// reads kernels: the most CTAs of 4 warps an SM holds (the window is static shared memory, so ask for the largest carveout)
+static int search_reads_grid(fxg_ctx *ctx, int64_t n_items) {
+    static int per_sm[2] = {0, 0};
+    if (!per_sm[0]) {
+        const void *k[2] = {(const void *)search_reads_kernel<S_COUNT>, (const void *)search_reads_kernel<S_ALL>};
+        for (int i = 0; i < 2; ++i) {
+            cudaFuncSetAttribute(k[i], cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+            int nb = 0;
+            if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k[i], RW * 32, 0) != cudaSuccess || nb < 1) nb = 1;
+            per_sm[i] = nb;
+        }
+    }
+    int64_t blocks = (n_items + RW - 1) / RW;
+    const int64_t maxb = (int64_t)ctx->sm_count * per_sm[0];
+    if (blocks > maxb) blocks = maxb;
+    return blocks < 1 ? 1 : (int)blocks;
+}
+
+extern "C" int fxg_search_reads_host(fxg_ctx *ctx, const fxg_file *f, const fxg_fastq_row *d_rows, int64_t n_rows,
+                                     const uint8_t *pattern, int32_t m, int strands, fxg_search_hit **out, int64_t *n_out) {
+    if (!ctx && fxg_device_count() == 0) {
+        fxg_set_error("no CUDA device available; libfxg has no CPU fallback");
+        return FXG_ENODEV;
+    }
+    FXG_CHECK_ARG(ctx && f && out && n_out && pattern && n_rows >= 0, "bad arguments");
+    FXG_CHECK_ARG(m >= 1 && m <= FXG_SEARCH_MAX_PATTERN, "pattern length must be 1 .. FXG_SEARCH_MAX_PATTERN");
+    FXG_CHECK_ARG(strands >= 1 && strands <= 3, "strands must be FXG_SEARCH_PLUS, FXG_SEARCH_MINUS or both");
+    FXG_CHECK_ARG(n_rows == 0 || d_rows, "d_rows == NULL");
+    *out = nullptr;
+    *n_out = 0;
+    FXG_LOCK(ctx);
+    FXG_CUDA(cudaSetDevice(ctx->device));
+    fxg_search_hit *h = nullptr;
+    int64_t n_hits = 0;
+    if (n_rows > 0) {
+        // misc: n_items per tile | zeros | tile_off (n_tiles + 1) | pattern
+        const int64_t n_tiles = (n_rows + 31) / 32;
+        const size_t tb = (size_t)n_tiles * 8;
+        int rc = ctx->misc.reserve(tb * 3 + 8 + SPB + 64);
+        if (rc) return rc;
+        int64_t *d_nit = (int64_t *)ctx->misc.ptr, *d_zero = d_nit + n_tiles, *d_toff = d_zero + n_tiles;
+        uint8_t *d_pat = (uint8_t *)(d_toff + n_tiles + 1);
+        FXG_CUDA(cudaMemcpyAsync(d_pat, pattern, (size_t)m, cudaMemcpyHostToDevice, ctx->stream));
+        FXG_CUDA(cudaMemsetAsync(d_zero, 0, tb, ctx->stream));
+        ReadSearchArgs A;
+        memset(&A, 0, sizeof(A));
+        A.file = f->d; A.fsize = f->size; A.rows = d_rows; A.n_rows = n_rows; A.n_tiles = n_tiles;
+        A.m = m; A.strands = strands; A.pattern = d_pat; A.tile_off = d_toff;
+        ctx->launches += 1;
+        search_reads_plan_kernel<<<(unsigned)((n_tiles + 7) / 8), 256, 0, ctx->stream>>>(A, d_nit);
+        FXG_CUDA(cudaGetLastError());
+        int64_t n_items = 0;
+        if ((rc = fxg_extract_plan_dev(ctx, d_zero, d_nit, n_tiles, d_toff, &n_items))) return rc;     // synchronises
+        // search scratch: tot | zeros | hit_off (n_items + 1)
+        if ((rc = ctx->search.reserve((size_t)n_items * 24 + 8 + 64))) return rc;
+        A.tot = (int64_t *)ctx->search.ptr;
+        int64_t *d_zero2 = A.tot + n_items, *d_hoff = d_zero2 + n_items;
+        A.hit_off = d_hoff;
+        const int grid = search_reads_grid(ctx, n_items);
+        {
+            FxgProfScope prof(ctx, FXG_PROF_GATHER);
+            search_reads_kernel<S_COUNT><<<grid, RW * 32, 0, ctx->stream>>>(A);
+        }
+        FXG_CUDA(cudaGetLastError());
+        rc = collect_hits(ctx, n_items, A.tot, d_zero2, d_hoff, [&](fxg_search_hit *o) {
+            A.out = o;
+            search_reads_kernel<S_ALL><<<grid, RW * 32, 0, ctx->stream>>>(A);
+        }, &h, &n_hits);
+        if (rc) return rc;
     }
     if (!h) {
         h = (fxg_search_hit *)malloc(sizeof(fxg_search_hit));

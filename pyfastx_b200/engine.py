@@ -399,6 +399,20 @@ class Engine:
         check(lib().fxg_search_host(self.ctx, dfile.handle, drows.devptr, drows.n_rows, rp, sp, ep, int(flags), nq,
                                     pat, len(pat), int(strands), _cabi.SEARCH_FIRST if first else _cabi.SEARCH_ALL,
                                     C.byref(out), C.byref(n)))
+        return self._take_hits(out, n)
+
+    def search_reads(self, dfile, drows, pattern, strands=_cabi.SEARCH_PLUS):
+        """Exact pattern search (K8 on reads) in every FASTQ read of drows; a read's haystack is its raw sequence line
+        (Read.seq).  -> SEARCH_HIT array of (query = read index, start, minus) in (query, start, minus) order."""
+        pat = bytes(pattern)
+        out = C.c_void_p()
+        n = C.c_int64(0)
+        check(lib().fxg_search_reads_host(self.ctx, dfile.handle, drows.devptr, drows.n_rows, pat, len(pat), int(strands),
+                                          C.byref(out), C.byref(n)))
+        return self._take_hits(out, n)
+
+    @staticmethod
+    def _take_hits(out, n):
         hits = np.zeros(n.value, dtype=_cabi.SEARCH_HIT)
         if n.value:
             C.memmove(hits.ctypes.data, out.value, n.value * _cabi.SEARCH_HIT.itemsize)

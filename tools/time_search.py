@@ -1,11 +1,13 @@
 #!/usr/bin/env python3
 """Time pattern search (K8) on the GPU, after verifying what it returns.
 
-    python tools/time_search.py [--steps 10] [--warmup 2] [--records 1000000] [--big-mb 250] [--out FILE]
+    python tools/time_search.py [--steps 10] [--warmup 2] [--records 1000000] [--big-mb 250] [--reads 126000000]
+                                [--sections locate,search,reads] [--profile] [--out FILE]
 
-Inputs are generated in HBM with fxg_synth_fasta_dev:
+Inputs are generated in HBM with fxg_synth_fasta_dev / fxg_synth_fastq_dev:
     c2   the bench's C2 shape: 1 M FASTA records of U[9000, 11000] bp at 80 columns (~10.2 GB)
     big  one record of --big-mb million bases at 80 columns
+    c4   the C4 shape: --reads FASTQ reads of 150 bp (~41.5 GB), scanned with fastq_scan
 
 Timed (CUDA events on the search's stream around `steps` consecutive calls, each of which ends in a host
 synchronisation, divided by `steps`):
@@ -13,6 +15,14 @@ synchronisation, divided by `steps`):
               "both"; GB/s is file bytes over call time, and its fraction of the H100 SXM's 3.35 TB/s data-sheet figure
     search    Sequence.search's call (first hit of one query) on the big record, against the path it replaces: extract
               the record to the host, decode it, str.find
+    reads     every occurrence in every C4 read (what Fastq.locate runs) of the same two patterns on "+" and "both",
+              alternating in the same call with the stand-in route it replaces: one-line FASTA rows over the same
+              reads through fxg_search_host.  fraction_of_byte_floor: the time to move the 32-byte sectors covering
+              every read's sequence plus 32 B per row at 3.35 TB/s, over the call time.  --profile: instead of the
+              timings, torch.profiler device time of the new kernels (plan, count, emit)
+
+Reads: every reported hit's window, fetched with fxg_reads_host, equals the pattern (or its reverse complement), and
+the per-read hit counts of the first 200,000 reads equal host bytes.find counts on those reads' bytes.
 
 Before any time is printed: every reported C2 hit's window, extracted with fxg_extract_host, equals the pattern (or its
 reverse complement on the minus strand), and the per-record hit counts of the first 20,000 records equal those found in
@@ -34,6 +44,7 @@ HBM_TBS = 3.35
 RARE = b"ACGTTGCATGCA"
 ECORI = b"GAATTC"
 N_ORACLE = 20000
+N_ORACLE_READS = 200000
 
 
 def gpu_info():
@@ -104,12 +115,117 @@ def verify_c2(eng, f, off, drows, rows, pat, hits):
     return int(exp.sum())
 
 
+def digits_upto(i):
+    total, lo, d = 0, 1, 1
+    while lo <= i:
+        hi = lo * 10 - 1
+        total += (min(i, hi) - lo + 1) * d
+        lo *= 10
+        d += 1
+    return total
+
+
+def verify_reads(eng, f, rows, pat, hits):
+    """hit windows through fxg_reads_host; per-read counts of the first reads against host bytes.find"""
+    from oracle import fxo
+    lut = fxo.complement_lut()
+    rc = bytes(lut[np.frombuffer(pat, np.uint8)][::-1])
+    m = len(pat)
+    q, st, mi = hits["query"], hits["start"], hits["minus"].astype(bool)
+    if q.size:
+        win, _ = eng.gather_ranges(f, rows["soff"][q] + st, np.full(q.size, m, np.int64))
+        want = np.where(mi[:, None], np.frombuffer(rc, np.uint8)[None, :], np.frombuffer(pat, np.uint8)[None, :])
+        assert np.array_equal(win.reshape(-1, m), want), "a reported hit's window differs from the pattern"
+    n = min(N_ORACLE_READS, len(rows))
+    hb = f.download(0, int(rows["qoff"][n - 1] + rows["rlen"][n - 1] + 1)).tobytes()
+    orows, _, _ = fxo.fastq_scan(hb)
+    assert len(orows) == n and np.array_equal(orows["soff"], rows["soff"][:n])
+    exp = np.zeros((n, 2), dtype=np.int64)
+    for i in range(n):
+        s = int(orows["soff"][i])
+        h = hb[s:s + int(orows["rlen"][i])]
+        for k, p in ((0, pat), (1, rc)):
+            j = h.find(p)
+            while j >= 0:
+                exp[i, k] += 1
+                j = h.find(p, j + 1)
+    sel = q < n
+    got = np.zeros((n, 2), dtype=np.int64)
+    np.add.at(got, (q[sel], mi[sel].astype(np.int64)), 1)
+    assert np.array_equal(got, exp), "hit counts of the first reads differ from host bytes.find"
+    return int(exp.sum())
+
+
+def section_reads(a, eng, stream, res):
+    """Fastq.locate's call on the C4 shape, against the stand-in route: one-line FASTA rows over the same reads
+    through fxg_search_host"""
+    import torch
+    from pyfastx_b200 import _cabi
+    L = _cabi.lib()
+    n = a.reads
+    f = eng.alloc_file(n * (5 + 11 + 1 + 150 + 1 + 2 + 150 + 1) + digits_upto(n))
+    _cabi.check(L.fxg_synth_fastq_dev(eng.ctx, 20240602, n, 0, 150, None, f.devptr))
+    eng.sync()
+    rows, st, drows = eng.fastq_scan(f, keep_device_rows=True)
+    assert len(rows) == n
+    # bytes the search has to read at the least: the 32-byte sectors covering every read's sequence, and its row
+    soff, rlen = rows["soff"], rows["rlen"]
+    floor = int(((((soff + rlen + 31) >> 5) - (soff >> 5)) * 32).sum()) + 32 * n
+    fr = np.zeros(n, dtype=_cabi.FASTA_ROW)
+    fr["boff"], fr["blen"], fr["slen"], fr["llen"] = soff, rlen, rlen, rlen + 1
+    fr["elen"], fr["norm"] = 1, 1
+    fr["pad"][:, 0] = 1
+    fdrows = eng.upload_rows(fr)
+    del fr
+    out = res["reads"] = {"file_gb": f.size / 1e9, "reads": n, "bases": int(st["total_len"]),
+                          "byte_floor_gb": floor / 1e9, "byte_floor_ms_at_3.35TBps": round(floor / (HBM_TBS * 1e12) * 1e3, 2)}
+    both = _cabi.SEARCH_PLUS | _cabi.SEARCH_MINUS
+    for name, pat in (("rare_12mer", RARE), ("GAATTC", ECORI)):
+        hits = eng.search_reads(f, drows, pat, both)
+        checked = verify_reads(eng, f, rows, pat, hits)
+        stand = eng.search(f, fdrows, None, None, None, 0, pat, both)
+        assert np.array_equal(stand, hits), "the stand-in route finds other hits"
+        del hits, stand
+        for strand, mask in () if a.profile else (("+", _cabi.SEARCH_PLUS), ("both", both)):
+            new = lambda: eng.search_reads(f, drows, pat, mask)
+            old = lambda: eng.search(f, fdrows, None, None, None, 0, pat, mask)
+            for _ in range(a.warmup):
+                new(); old()
+            n_hits = len(new())
+            tn, to = [], []
+            for _ in range(3):                                  # alternating, in the same call
+                tn.append(timed(stream, a.steps, new))
+                to.append(timed(stream, a.steps, old))
+            med, medo = float(np.median(tn)), float(np.median(to))
+            out["%s %s" % (name, strand)] = {
+                "hits": n_hits, "ms_median": round(med, 3), "ms_min": round(min(tn), 3), "ms_max": round(max(tn), 3),
+                "file_GBps": round(f.size / (med * 1e-3) / 1e9, 1),
+                "fraction_of_byte_floor": round(floor / (HBM_TBS * 1e12) * 1e3 / med, 3),
+                "standin_fxg_search_host_ms_median": round(medo, 3), "speedup_vs_standin": round(medo / med, 2),
+                "host_checked_hits_first_%d_reads" % N_ORACLE_READS: checked}
+    if a.profile:
+        from torch.profiler import ProfilerActivity, profile
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for pat in (RARE, ECORI):
+                eng.search_reads(f, drows, pat, _cabi.SEARCH_PLUS)
+            torch.cuda.synchronize()
+        kern = {}
+        for ev in prof.key_averages():
+            if "search_reads" in ev.key or "Memcpy DtoH" in ev.key:
+                kern[ev.key] = {"calls": ev.count, "device_ms_total": round(ev.device_time_total / 1e3, 3)}
+        out["profile_rare_then_GAATTC_plus"] = kern
+    fdrows.free(); drows.free(); f.free()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--records", type=int, default=1000000)
     ap.add_argument("--big-mb", type=int, default=250)
+    ap.add_argument("--reads", type=int, default=126000000)
+    ap.add_argument("--sections", default="locate,search,reads")
+    ap.add_argument("--profile", action="store_true", help="reads: torch.profiler device time of each new kernel only")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     import torch
@@ -119,62 +235,71 @@ def main():
     stream = torch.cuda.Stream()
     eng.set_stream(stream.cuda_stream)
     res = {"gpu": gpu_info(), "device": torch.cuda.get_device_name(0), "locate": {}, "search": {}}
+    sections = a.sections.split(",")
+    if a.profile:
+        section_reads(a, eng, stream, res)
+        sections = []
 
-    lengths = synth.fasta_lengths(a.records, 20240601, 9000, 11000)
-    f, off = make_fasta(eng, lengths)
-    rows, st, drows = eng.fasta_scan(f, keep_device_rows=True)
-    assert len(rows) == a.records
-    res["c2"] = {"file_gb": f.size / 1e9, "records": len(rows), "bases": int(st["total_len"])}
-    both = _cabi.SEARCH_PLUS | _cabi.SEARCH_MINUS
-    for name, pat in (("rare_12mer", RARE), ("GAATTC", ECORI)):
-        hits = eng.search(f, drows, None, None, None, 0, pat, both)
-        checked = verify_c2(eng, f, off, drows, rows, pat, hits)
-        for strand, mask in (("+", _cabi.SEARCH_PLUS), ("both", both)):
-            call = lambda: eng.search(f, drows, None, None, None, 0, pat, mask)
+    if "locate" in sections:
+        lengths = synth.fasta_lengths(a.records, 20240601, 9000, 11000)
+        f, off = make_fasta(eng, lengths)
+        rows, st, drows = eng.fasta_scan(f, keep_device_rows=True)
+        assert len(rows) == a.records
+        res["c2"] = {"file_gb": f.size / 1e9, "records": len(rows), "bases": int(st["total_len"])}
+        both = _cabi.SEARCH_PLUS | _cabi.SEARCH_MINUS
+        for name, pat in (("rare_12mer", RARE), ("GAATTC", ECORI)):
+            hits = eng.search(f, drows, None, None, None, 0, pat, both)
+            checked = verify_c2(eng, f, off, drows, rows, pat, hits)
+            for strand, mask in (("+", _cabi.SEARCH_PLUS), ("both", both)):
+                call = lambda: eng.search(f, drows, None, None, None, 0, pat, mask)
+                for _ in range(a.warmup):
+                    call()
+                n_hits = len(call())
+                ms = [timed(stream, a.steps, call) for _ in range(3)]
+                med = float(np.median(ms))
+                gbs = f.size / (med * 1e-3) / 1e9
+                res["locate"]["%s %s" % (name, strand)] = {
+                    "hits": n_hits, "ms_median": round(med, 3), "ms_min": round(min(ms), 3), "ms_max": round(max(ms), 3),
+                    "file_GBps": round(gbs, 1), "fraction_of_3.35TBps": round(gbs / 1e3 / HBM_TBS, 3),
+                    "oracle_checked_hits_first_%d_records" % N_ORACLE: checked}
+        drows.free(); f.free()
+
+    if "search" in sections:
+        big = np.array([a.big_mb * 1000000], dtype=np.int64)
+        f, off = make_fasta(eng, big, seed=7)
+        rows, _, drows = eng.fasta_scan(f, keep_device_rows=True)
+        slen = int(rows["slen"][0])
+        rid, s0, e0 = np.array([0]), np.array([0]), np.array([slen])
+        seq_tail = eng.extract(f, drows, rid, e0 - 40, e0, np.zeros(1, np.int32))[0].tobytes()
+        for name, pat in (("rare_12mer", RARE), ("near_end_20mer", seq_tail[5:25])):
+            def gpu_first(strands=_cabi.SEARCH_PLUS):
+                h = eng.search(f, drows, rid, s0, e0, 0, pat, strands, first=True)
+                return int(h["start"][0]) + 1 if h.size else None
+            def host_find():
+                k = eng.extract_one(f, drows, 0, 0, slen, 0).decode("latin-1").find(pat.decode())
+                return k + 1 if k >= 0 else None
+            g, hst = gpu_first(), host_find()
+            assert g == hst, (name, g, hst)
             for _ in range(a.warmup):
-                call()
-            n_hits = len(call())
-            ms = [timed(stream, a.steps, call) for _ in range(3)]
-            med = float(np.median(ms))
-            gbs = f.size / (med * 1e-3) / 1e9
-            res["locate"]["%s %s" % (name, strand)] = {
-                "hits": n_hits, "ms_median": round(med, 3), "ms_min": round(min(ms), 3), "ms_max": round(max(ms), 3),
-                "file_GBps": round(gbs, 1), "fraction_of_3.35TBps": round(gbs / 1e3 / HBM_TBS, 3),
-                "oracle_checked_hits_first_%d_records" % N_ORACLE: checked}
-    drows.free(); f.free()
-
-    big = np.array([a.big_mb * 1000000], dtype=np.int64)
-    f, off = make_fasta(eng, big, seed=7)
-    rows, _, drows = eng.fasta_scan(f, keep_device_rows=True)
-    slen = int(rows["slen"][0])
-    rid, s0, e0 = np.array([0]), np.array([0]), np.array([slen])
-    seq_tail = eng.extract(f, drows, rid, e0 - 40, e0, np.zeros(1, np.int32))[0].tobytes()
-    for name, pat in (("rare_12mer", RARE), ("near_end_20mer", seq_tail[5:25])):
-        def gpu_first(strands=_cabi.SEARCH_PLUS):
-            h = eng.search(f, drows, rid, s0, e0, 0, pat, strands, first=True)
-            return int(h["start"][0]) + 1 if h.size else None
-        def host_find():
-            k = eng.extract_one(f, drows, 0, 0, slen, 0).decode("latin-1").find(pat.decode())
-            return k + 1 if k >= 0 else None
-        g, hst = gpu_first(), host_find()
-        assert g == hst, (name, g, hst)
-        for _ in range(a.warmup):
-            gpu_first()
-        tg = []
-        for _ in range(3):
-            t0 = time.perf_counter()
-            for _ in range(a.steps):
                 gpu_first()
-            tg.append((time.perf_counter() - t0) / a.steps * 1e3)
-        th = []
-        for _ in range(3):
-            t0 = time.perf_counter()
-            host_find()
-            th.append((time.perf_counter() - t0) * 1e3)
-        res["search"][name] = {"record_bases": slen, "answer": g, "gpu_ms_median": round(float(np.median(tg)), 3),
-                               "extract_decode_find_ms_median": round(float(np.median(th)), 1),
-                               "speedup": round(float(np.median(th)) / float(np.median(tg)), 1)}
-    drows.free(); f.free()
+            tg = []
+            for _ in range(3):
+                t0 = time.perf_counter()
+                for _ in range(a.steps):
+                    gpu_first()
+                tg.append((time.perf_counter() - t0) / a.steps * 1e3)
+            th = []
+            for _ in range(3):
+                t0 = time.perf_counter()
+                host_find()
+                th.append((time.perf_counter() - t0) * 1e3)
+            res["search"][name] = {"record_bases": slen, "answer": g, "gpu_ms_median": round(float(np.median(tg)), 3),
+                                   "extract_decode_find_ms_median": round(float(np.median(th)), 1),
+                                   "speedup": round(float(np.median(th)) / float(np.median(tg)), 1)}
+        drows.free(); f.free()
+    if "reads" in sections:
+        _cabi.lib().fxg_pool_trim()                         # the freed C2 / big buffers stay pooled: give them back
+        section_reads(a, eng, stream, res)
     s = json.dumps(res, indent=1)
     if a.out:
         with open(a.out, "w") as fh:
