@@ -295,7 +295,8 @@ int fxg_composition_host(fxg_ctx *ctx, const fxg_file *f, const fxg_fasta_row *d
 #define FXG_SEARCH_MAX_PATTERN  1024
 enum { FXG_SEARCH_PLUS = 1, FXG_SEARCH_MINUS = 2 };          /* strands mask */
 enum { FXG_SEARCH_ALL = 0, FXG_SEARCH_FIRST = 1 };            /* mode */
-typedef struct fxg_search_hit { int64_t query, start; int32_t minus, pad; } fxg_search_hit;   /* 24 B */
+/* 24 B; mismatches: the substitutions of a hit of the search with mismatches below, 0 for the exact search */
+typedef struct fxg_search_hit { int64_t query, start; int32_t minus, mismatches; } fxg_search_hit;
 int fxg_search_host(fxg_ctx *ctx, const fxg_file *f, const fxg_fasta_row *d_rows, int64_t n_rows,
                     const int64_t *row_id, const int64_t *s, const int64_t *e, int32_t flags, int64_t nq,
                     const uint8_t *pattern, int32_t m, int strands, int mode,
@@ -312,6 +313,26 @@ int fxg_search_host(fxg_ctx *ctx, const fxg_file *f, const fxg_fasta_row *d_rows
  * Synchronises after sizing the work, after counting the hits and at the end. */
 int fxg_search_reads_host(fxg_ctx *ctx, const fxg_file *f, const fxg_fastq_row *d_rows, int64_t n_rows,
                           const uint8_t *pattern, int32_t m, int strands, fxg_search_hit **out, int64_t *n_out);
+
+/* Search with mismatches: every start within max_mismatches substitutions of the pattern.  The haystacks are exactly
+ * those of the exact entry points above: for fxg_search_approx_host the bytes extraction returns for the query (10 / 13 /
+ * 32 stripped, FXG_X_UPPER applied if set), for fxg_search_reads_approx_host the raw rlen bytes at soff (Read.seq).
+ * A hit is a start i with i + m <= len and at most max_mismatches positions j where hay[i + j] != pattern[j]
+ * (Hamming distance, substitutions only; byte for byte and case-sensitive, so 'N' against 'A' is a mismatch).  The
+ * minus strand compares against the pattern's reverse complement under the extraction table.  A window never extends
+ * past its haystack's end: no partial window at a record's or read's end is reported, even if counting the missing
+ * bytes as mismatches would keep it within the limit.  Every qualifying start is reported, overlapping ones included,
+ * in (query, start, minus) order, deterministically; hit.mismatches is its count (0 .. max_mismatches) against the
+ * strand it matched.  The exact entry points write 0 there.  max_mismatches = 0 gives exactly the exact search's hits.
+ * 1 <= m <= FXG_SEARCH_MAX_PATTERN and 0 <= max_mismatches < m, else FXG_EINVAL.  There is no first-hit mode.
+ * Arguments, row_id == NULL, output and synchronisation are as for fxg_search_host / fxg_search_reads_host. */
+int fxg_search_approx_host(fxg_ctx *ctx, const fxg_file *f, const fxg_fasta_row *d_rows, int64_t n_rows,
+                           const int64_t *row_id, const int64_t *s, const int64_t *e, int32_t flags, int64_t nq,
+                           const uint8_t *pattern, int32_t m, int32_t max_mismatches, int strands,
+                           fxg_search_hit **out, int64_t *n_out);
+int fxg_search_reads_approx_host(fxg_ctx *ctx, const fxg_file *f, const fxg_fastq_row *d_rows, int64_t n_rows,
+                                 const uint8_t *pattern, int32_t m, int32_t max_mismatches, int strands,
+                                 fxg_search_hit **out, int64_t *n_out);
 
 /* ---- K5: batched FASTQ read fetch ----------------------------------------------------------
  * Replaces pyfastx_read_random_reader + the seq/qual getters (src/read.c:37-45,152-167,

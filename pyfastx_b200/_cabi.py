@@ -54,7 +54,7 @@ class FastqMeta(C.Structure):
 
 
 COMP_ROW = np.dtype([("seqid", "<i8"), ("abc", "<i8"), ("num", "<i8")])
-SEARCH_HIT = np.dtype([("query", "<i8"), ("start", "<i8"), ("minus", "<i4"), ("pad", "<i4")])   # fxg_search_hit
+SEARCH_HIT = np.dtype([("query", "<i8"), ("start", "<i8"), ("minus", "<i4"), ("mismatches", "<i4")])   # fxg_search_hit
 
 SEARCH_PIECE, SEARCH_MAX_PATTERN = 4096, 1024                     # FXG_SEARCH_PIECE, FXG_SEARCH_MAX_PATTERN
 SEARCH_PLUS, SEARCH_MINUS = 1, 2
@@ -128,6 +128,8 @@ SIGNATURES = {
     "fxg_composition_host": (i32, [vp, vp, vp, i64, vp, vp, vp, vp, i64, vp]),
     "fxg_search_host": (i32, [vp, vp, vp, i64, vp, vp, vp, i32, i64, vp, i32, i32, i32, P(vp), P(i64)]),
     "fxg_search_reads_host": (i32, [vp, vp, vp, i64, vp, i32, i32, P(vp), P(i64)]),
+    "fxg_search_approx_host": (i32, [vp, vp, vp, i64, vp, vp, vp, i32, i64, vp, i32, i32, i32, P(vp), P(i64)]),
+    "fxg_search_reads_approx_host": (i32, [vp, vp, vp, i64, vp, i32, i32, i32, P(vp), P(i64)]),
     "fxg_reads_dev": (i32, [vp, vp, vp, i64, vp, i64, i32, vp, vp, vp, i64, P(i64)]),
     "fxg_reads_host": (i32, [vp, vp, vp, i64, vp, i64, i32, vp, vp, vp, i64]),
     "fxg_read_one_host": (i32, [vp, vp, vp, i64, i64, i32, i32, i64, vp, i64]),

@@ -83,6 +83,21 @@ def _locate_result(hits):
     return (hits["query"].astype(np.int64), hits["start"].astype(np.int64), hits["minus"].astype(bool))
 
 
+def _locate_approx_args(pattern, mismatches, strand):
+    """(pattern bytes, mismatches, strands mask) of a locate_approx call; TypeError for a mismatches that is not an
+    integer (a bool is not), ValueError for one outside 0 .. len(pattern) - 1"""
+    data, strands = _locate_args(pattern, strand)
+    if isinstance(mismatches, (bool, np.bool_)) or not isinstance(mismatches, (int, np.integer)):
+        raise TypeError("mismatches must be an integer")
+    if not 0 <= mismatches < len(data):
+        raise ValueError("mismatches must be 0 .. len(pattern) - 1")
+    return data, int(mismatches), strands
+
+
+def _locate_approx_result(hits):
+    return _locate_result(hits) + (hits["mismatches"].astype(np.int32),)
+
+
 def _gzip_header_len(comp):
     """bytes of the gzip member header (RFC 1952) in front of the deflate data"""
     flg = int(comp[3])
@@ -483,6 +498,18 @@ class Fasta:
         self._need_index()
         return _locate_result(self._st.engine.search(self._st.dfile, self._drows, None, None, None, self._flags(), data,
                                                      strands))
+
+    def locate_approx(self, pattern, mismatches, strand="+"):
+        """Every start in every record where `pattern` matches with at most `mismatches` substituted bytes (Hamming
+        distance; byte for byte and case-sensitive, so N against A is a mismatch), found by the search kernel on the
+        resident file.  Strand and uppercase=True as for locate; a match never runs past its record's end.
+        0 <= mismatches < len(pattern); mismatches = 0 gives locate's hits.
+        -> (row_id int64, start int64, minus bool, mismatches int32) arrays sorted by (row_id, start, minus); the last
+        holds each hit's count of mismatches against the strand it matched."""
+        data, k, strands = _locate_approx_args(pattern, mismatches, strand)
+        self._need_index()
+        return _locate_approx_result(self._st.engine.search_approx(self._st.dfile, self._drows, None, None, None,
+                                                                   self._flags(), data, k, strands))
 
     # ---- reference methods -------------------------------------------------------------------------
     def fetch(self, chrom, intervals, strand="+"):
@@ -899,6 +926,17 @@ class Fastq:
         data, strands = _locate_args(pattern, strand)
         self.build_index()
         return _locate_result(self._st.engine.search_reads(self._st.dfile, self._drows, data, strands))
+
+    def locate_approx(self, pattern, mismatches, strand="+"):
+        """Every start in every read's sequence (exactly Read.seq) where `pattern` matches with at most `mismatches`
+        substituted bytes (Hamming distance; byte for byte and case-sensitive, so N against A is a mismatch), found by
+        the search kernel on the resident file.  Strand as for locate; a match never runs past its read's end.
+        0 <= mismatches < len(pattern); mismatches = 0 gives locate's hits.
+        -> (read_id int64, start int64, minus bool, mismatches int32) arrays sorted by (read_id, start, minus); the last
+        holds each hit's count of mismatches against the strand it matched."""
+        data, k, strands = _locate_approx_args(pattern, mismatches, strand)
+        self.build_index()
+        return _locate_approx_result(self._st.engine.search_reads_approx(self._st.dfile, self._drows, data, k, strands))
 
     def _calc_composition(self):
         """pyfastx_fastq_calc_composition (src/fastq.c:663-795): base totals, min / max length and quality, phred

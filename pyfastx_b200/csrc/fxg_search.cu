@@ -78,11 +78,40 @@ __device__ __forceinline__ bool rest_equal(const uint8_t *h, int i, const uint8_
     }
     return true;
 }
+// bytes of x that are not zero
+__device__ __forceinline__ int nonzero_bytes(uint32_t x) { return __popc((((x & 0x7f7f7f7fu) + 0x7f7f7f7fu) | x) & 0x80808080u); }
+
+// The per-start test, on a start's first (up to) four bytes w against the pattern's p, both masked to m bytes: first(w,
+// p); for a start that passed and m > 4, on the whole window: rest(h, i, P, m).  mismatches(h, i, P, m) is what a hit
+// reports.  ExactTest is K8's byte-for-byte test.
+struct ExactTest {
+    __device__ __forceinline__ bool first(uint32_t w, uint32_t p) const { return w == p; }
+    __device__ __forceinline__ bool rest(const uint8_t *h, int i, const uint8_t *P, int m) const { return rest_equal(h, i, P, m); }
+    __device__ __forceinline__ int mismatches(const uint8_t *, int, const uint8_t *, int) const { return 0; }
+};
+// At most k substituted bytes (Hamming distance): XOR word by word, count the bytes that differ, stop at the first word
+// that takes the count past k.  On uniform random bases 3 of 4 bytes differ, so a start costs about (k + 1) / 3 words.
+struct ApproxTest {
+    int k;
+    __device__ __forceinline__ int mismatches(const uint8_t *h, int i, const uint8_t *P, int m) const {
+        const uint32_t *pw = reinterpret_cast<const uint32_t *>(P);
+        int n = 0;
+        for (int j = 0; j < m && n <= k; j += 4) {
+            uint32_t d = word_at(h, i + j) ^ pw[j >> 2];
+            if (m - j < 4) d &= (1u << (8 * (m - j))) - 1u;
+            n += nonzero_bytes(d);
+        }
+        return n;
+    }
+    __device__ __forceinline__ bool first(uint32_t w, uint32_t p) const { return nonzero_bytes(w ^ p) <= k; }
+    __device__ __forceinline__ bool rest(const uint8_t *h, int i, const uint8_t *P, int m) const { return mismatches(h, i, P, m) <= k; }
+};
 
 // Runs work item p of query q on the strands in `strands` (bit 0 plus, bit 1 minus).  S_COUNT adds the lane's hits to
 // cp / cm; S_ALL writes every hit from A.out[out_pos] on; S_FIRST writes the first hit to A.out[out_pos] and returns.
-template <int MODE>
-__device__ void run_item(const SearchArgs &A, int64_t q, int64_t p, int strands, uint8_t *__restrict__ hb,
+// T: the per-start test (ExactTest, ApproxTest).
+template <int MODE, class T>
+__device__ void run_item(const SearchArgs &A, const T &test, int64_t q, int64_t p, int strands, uint8_t *__restrict__ hb,
                          const uint8_t *__restrict__ pat, const uint8_t *__restrict__ rc, int lane, int64_t out_pos,
                          int64_t &cp, int64_t &cm) {
     int64_t s, e;
@@ -203,8 +232,8 @@ __device__ void run_item(const SearchArgs &A, int64_t q, int64_t p, int strands,
                     const int i = i0 + k;
                     if (i < nt) {
                         const uint32_t w = (k ? __funnelshift_r(W0, W1, 8 * k) : W0) & pmask;
-                        if (want_p && w == pp && (m <= 4 || rest_equal(hb, i, pat, m))) hp |= 1u << k;
-                        if (want_m && w == pm && (m <= 4 || rest_equal(hb, i, rc, m))) hm |= 1u << k;
+                        if (want_p && test.first(w, pp) && (m <= 4 || test.rest(hb, i, pat, m))) hp |= 1u << k;
+                        if (want_m && test.first(w, pm) && (m <= 4 || test.rest(hb, i, rc, m))) hm |= 1u << k;
                     }
                 }
                 if (MODE == S_COUNT) {
@@ -222,8 +251,8 @@ __device__ void run_item(const SearchArgs &A, int64_t q, int64_t p, int strands,
                         int64_t o = cursor + (inc - n);
 #pragma unroll
                         for (int k = 0; k < 4; ++k) {                         // (start, minus) order
-                            if ((hp >> k) & 1u) { fxg_search_hit *h = A.out + o++; h->query = q; h->start = start0 + i0 + k; h->minus = 0; h->pad = 0; }
-                            if ((hm >> k) & 1u) { fxg_search_hit *h = A.out + o++; h->query = q; h->start = start0 + i0 + k; h->minus = 1; h->pad = 0; }
+                            if ((hp >> k) & 1u) { fxg_search_hit *h = A.out + o++; h->query = q; h->start = start0 + i0 + k; h->minus = 0; h->mismatches = test.mismatches(hb, i0 + k, pat, m); }
+                            if ((hm >> k) & 1u) { fxg_search_hit *h = A.out + o++; h->query = q; h->start = start0 + i0 + k; h->minus = 1; h->mismatches = test.mismatches(hb, i0 + k, rc, m); }
                         }
                         cursor += __shfl_sync(0xffffffffu, inc, 31);
                     }
@@ -233,7 +262,7 @@ __device__ void run_item(const SearchArgs &A, int64_t q, int64_t p, int strands,
                     if (bal) {
                         if (lane == __ffs(bal) - 1) {
                             fxg_search_hit *o = A.out + out_pos;
-                            o->query = q; o->start = start0 + i0 + __ffs(h) - 1; o->minus = want_m ? 1 : 0; o->pad = 0;
+                            o->query = q; o->start = start0 + i0 + __ffs(h) - 1; o->minus = want_m ? 1 : 0; o->mismatches = 0;
                         }
                         return;
                     }
@@ -265,8 +294,9 @@ __global__ void search_items_kernel(SearchArgs A, int64_t *__restrict__ n_items)
     n_items[q] = n;
 }
 
-template <int MODE>
-__global__ void __launch_bounds__(SW * 32, 4) search_kernel(SearchArgs A) {
+// The count / emit / first-hit pass over the work items, with the per-start test T.
+template <int MODE, class T>
+__device__ __forceinline__ void search_items(const SearchArgs &A, const T &test) {
     __shared__ __align__(16) uint8_t s_pat[2][SPB];             // the pattern and its reverse complement
     __shared__ __align__(16) uint8_t s_hay[SW][SHB];
     const int m = A.m;
@@ -288,7 +318,7 @@ __global__ void __launch_bounds__(SW * 32, 4) search_kernel(SearchArgs A) {
                 if (A.item_off[mid] <= it) lo = mid; else hi = mid;
             }
             cp = cm = 0;
-            run_item<MODE>(A, lo, it - A.item_off[lo], A.strands, s_hay[warp], s_pat[0], s_pat[1], lane,
+            run_item<MODE>(A, test, lo, it - A.item_off[lo], A.strands, s_hay[warp], s_pat[0], s_pat[1], lane,
                            MODE == S_ALL ? A.hit_off[it] : 0, cp, cm);
             if (MODE == S_COUNT) {
 #pragma unroll
@@ -315,10 +345,18 @@ __global__ void __launch_bounds__(SW * 32, 4) search_kernel(SearchArgs A) {
             if (lane == 0) A.out[w].query = -1;
             __syncwarp();
             if (first >= 0)
-                run_item<S_FIRST>(A, q, first - A.item_off[q], 1 << st, s_hay[warp], s_pat[0], s_pat[1], lane, w, cp, cm);
+                run_item<S_FIRST>(A, test, q, first - A.item_off[q], 1 << st, s_hay[warp], s_pat[0], s_pat[1], lane, w, cp, cm);
             __syncwarp();
         }
     }
+}
+
+template <int MODE>
+__global__ void __launch_bounds__(SW * 32, 4) search_kernel(SearchArgs A) { search_items<MODE>(A, ExactTest{}); }
+// every start within max_mm substitutions; no first-hit mode
+template <int MODE>
+__global__ void __launch_bounds__(SW * 32, 4) search_approx_kernel(SearchArgs A, int max_mm) {
+    search_items<MODE>(A, ApproxTest{max_mm});
 }
 
 // ---- K8 on FASTQ reads ----------------------------------------------------------------------------------------------
@@ -385,9 +423,9 @@ __global__ void search_reads_plan_kernel(ReadSearchArgs A, int64_t *__restrict__
 }
 
 // Every warp runs a contiguous range of items.  S_COUNT writes each item's hits to A.tot; S_ALL re-runs the items with
-// hits and writes them from A.hit_off[item] on, in (read, start, minus) order.
-template <int MODE>
-__global__ void __launch_bounds__(RW * 32) search_reads_kernel(ReadSearchArgs A) {
+// hits and writes them from A.hit_off[item] on, in (read, start, minus) order.  T: the per-start test.
+template <int MODE, class T>
+__device__ __forceinline__ void search_reads_items(const ReadSearchArgs &A, const T &test) {
     __shared__ __align__(16) uint8_t s_pat[2][SPB];
     __shared__ __align__(16) uint8_t s_win[RW][RWIN + 16];      // + one word read past the last chunk
     __shared__ uint8_t s_map[RW][RCH];                           // chunk -> lane whose segment it holds
@@ -492,16 +530,16 @@ __global__ void __launch_bounds__(RW * 32) search_reads_kernel(ReadSearchArgs A)
 #pragma unroll
                     for (int q = 0; q < 16; ++q) {
                         const uint32_t w = ((q & 3) ? __funnelshift_r(W[q >> 2], W[(q >> 2) + 1], 8 * (q & 3)) : W[q >> 2]) & pmask;
-                        hp |= (uint32_t)(want_p && w == pp) << q;
-                        hm |= (uint32_t)(want_m && w == pm) << q;
+                        hp |= (uint32_t)(want_p && test.first(w, pp)) << q;
+                        hm |= (uint32_t)(want_m && test.first(w, pm)) << q;
                     }
                     hp &= valid;
                     hm &= valid;
                     if (m > 4) {
                         for (uint32_t x = hp; x; x &= x - 1u)
-                            if (!rest_equal(win, 16 * ci + __ffs(x) - 1, s_pat[0], m)) hp &= ~(x & (0u - x));
+                            if (!test.rest(win, 16 * ci + __ffs(x) - 1, s_pat[0], m)) hp &= ~(x & (0u - x));
                         for (uint32_t x = hm; x; x &= x - 1u)
-                            if (!rest_equal(win, 16 * ci + __ffs(x) - 1, s_pat[1], m)) hm &= ~(x & (0u - x));
+                            if (!test.rest(win, 16 * ci + __ffs(x) - 1, s_pat[1], m)) hm &= ~(x & (0u - x));
                     }
                 }
                 if (MODE == S_COUNT) {
@@ -520,8 +558,8 @@ __global__ void __launch_bounds__(RW * 32) search_reads_kernel(ReadSearchArgs A)
                         const int64_t rid = t * 32 + j, s0 = aj + k0;
                         for (uint32_t x = hp | hm; x; x &= x - 1u) {                // (start, minus) order
                             const int q = __ffs(x) - 1;
-                            if ((hp >> q) & 1u) { fxg_search_hit *h = A.out + o++; h->query = rid; h->start = s0 + q; h->minus = 0; h->pad = 0; }
-                            if ((hm >> q) & 1u) { fxg_search_hit *h = A.out + o++; h->query = rid; h->start = s0 + q; h->minus = 1; h->pad = 0; }
+                            if ((hp >> q) & 1u) { fxg_search_hit *h = A.out + o++; h->query = rid; h->start = s0 + q; h->minus = 0; h->mismatches = test.mismatches(win, 16 * ci + q, s_pat[0], m); }
+                            if ((hm >> q) & 1u) { fxg_search_hit *h = A.out + o++; h->query = rid; h->start = s0 + q; h->minus = 1; h->mismatches = test.mismatches(win, 16 * ci + q, s_pat[1], m); }
                         }
                         cursor += __shfl_sync(0xffffffffu, inc, 31);
                     }
@@ -536,6 +574,14 @@ __global__ void __launch_bounds__(RW * 32) search_reads_kernel(ReadSearchArgs A)
             if (lane == 0) A.tot[it] = cnt;
         }
     }
+}
+
+template <int MODE>
+__global__ void __launch_bounds__(RW * 32) search_reads_kernel(ReadSearchArgs A) { search_reads_items<MODE>(A, ExactTest{}); }
+// every start within max_mm substitutions
+template <int MODE>
+__global__ void __launch_bounds__(RW * 32) search_reads_approx_kernel(ReadSearchArgs A, int max_mm) {
+    search_reads_items<MODE>(A, ApproxTest{max_mm});
 }
 
 }  // namespace fxg
@@ -572,16 +618,17 @@ static int collect_hits(fxg_ctx *ctx, int64_t n_items, const int64_t *d_tot, int
     return FXG_OK;
 }
 
-extern "C" int fxg_search_host(fxg_ctx *ctx, const fxg_file *f, const fxg_fasta_row *d_rows, int64_t n_rows,
-                               const int64_t *row_id, const int64_t *s, const int64_t *e, int32_t flags, int64_t nq,
-                               const uint8_t *pattern, int32_t m, int strands, int mode, fxg_search_hit **out,
-                               int64_t *n_out) {
+// fxg_search_host (K8's exact test) and fxg_search_approx_host (approx: at most max_mm mismatches, mode FXG_SEARCH_ALL)
+static int search_host(fxg_ctx *ctx, const fxg_file *f, const fxg_fasta_row *d_rows, int64_t n_rows, const int64_t *row_id,
+                       const int64_t *s, const int64_t *e, int32_t flags, int64_t nq, const uint8_t *pattern, int32_t m,
+                       bool approx, int32_t max_mm, int strands, int mode, fxg_search_hit **out, int64_t *n_out) {
     if (!ctx && fxg_device_count() == 0) {
         fxg_set_error("no CUDA device available; libfxg has no CPU fallback");
         return FXG_ENODEV;
     }
     FXG_CHECK_ARG(ctx && f && out && n_out && pattern && nq >= 0 && n_rows >= 0, "bad arguments");
     FXG_CHECK_ARG(m >= 1 && m <= FXG_SEARCH_MAX_PATTERN, "pattern length must be 1 .. FXG_SEARCH_MAX_PATTERN");
+    FXG_CHECK_ARG(!approx || (max_mm >= 0 && max_mm < m), "max_mismatches must be 0 .. m - 1");
     FXG_CHECK_ARG(strands >= 1 && strands <= 3, "strands must be FXG_SEARCH_PLUS, FXG_SEARCH_MINUS or both");
     FXG_CHECK_ARG(mode == FXG_SEARCH_ALL || mode == FXG_SEARCH_FIRST, "mode must be FXG_SEARCH_ALL or FXG_SEARCH_FIRST");
     FXG_CHECK_ARG((flags & ~FXG_X_UPPER) == 0, "flags other than FXG_X_UPPER are not searchable");
@@ -628,13 +675,15 @@ extern "C" int fxg_search_host(fxg_ctx *ctx, const fxg_file *f, const fxg_fasta_
             A.hit_off = d_hoff;
             {
                 FxgProfScope prof(ctx, FXG_PROF_GATHER);
-                search_kernel<S_COUNT><<<search_grid(ctx, n_items), SW * 32, 0, ctx->stream>>>(A);
+                if (!approx) search_kernel<S_COUNT><<<search_grid(ctx, n_items), SW * 32, 0, ctx->stream>>>(A);
+                else search_approx_kernel<S_COUNT><<<search_grid(ctx, n_items), SW * 32, 0, ctx->stream>>>(A, max_mm);
             }
             FXG_CUDA(cudaGetLastError());
             if (mode == FXG_SEARCH_ALL) {
                 rc = collect_hits(ctx, n_items, A.tot, d_zero2, d_hoff, [&](fxg_search_hit *o) {
                     A.out = o;
-                    search_kernel<S_ALL><<<search_grid(ctx, n_items), SW * 32, 0, ctx->stream>>>(A);
+                    if (!approx) search_kernel<S_ALL><<<search_grid(ctx, n_items), SW * 32, 0, ctx->stream>>>(A);
+                    else search_approx_kernel<S_ALL><<<search_grid(ctx, n_items), SW * 32, 0, ctx->stream>>>(A, max_mm);
                 }, &h, &n_hits);
                 if (rc) return rc;
             } else {
@@ -666,32 +715,53 @@ extern "C" int fxg_search_host(fxg_ctx *ctx, const fxg_file *f, const fxg_fasta_
     return FXG_OK;
 }
 
-// reads kernels: the most CTAs of 4 warps an SM holds (the window is static shared memory, so ask for the largest carveout)
-static int search_reads_grid(fxg_ctx *ctx, int64_t n_items) {
+extern "C" int fxg_search_host(fxg_ctx *ctx, const fxg_file *f, const fxg_fasta_row *d_rows, int64_t n_rows,
+                               const int64_t *row_id, const int64_t *s, const int64_t *e, int32_t flags, int64_t nq,
+                               const uint8_t *pattern, int32_t m, int strands, int mode, fxg_search_hit **out,
+                               int64_t *n_out) {
+    return search_host(ctx, f, d_rows, n_rows, row_id, s, e, flags, nq, pattern, m, false, 0, strands, mode, out, n_out);
+}
+
+extern "C" int fxg_search_approx_host(fxg_ctx *ctx, const fxg_file *f, const fxg_fasta_row *d_rows, int64_t n_rows,
+                                      const int64_t *row_id, const int64_t *s, const int64_t *e, int32_t flags, int64_t nq,
+                                      const uint8_t *pattern, int32_t m, int32_t max_mismatches, int strands,
+                                      fxg_search_hit **out, int64_t *n_out) {
+    return search_host(ctx, f, d_rows, n_rows, row_id, s, e, flags, nq, pattern, m, true, max_mismatches,
+                       strands, FXG_SEARCH_ALL, out, n_out);
+}
+
+// reads kernels: the most CTAs of 4 warps an SM holds (the window is static shared memory, so ask for the largest
+// carveout); per_sm[0] for the exact kernels, per_sm[1] for the approximate ones
+static int search_reads_grid(fxg_ctx *ctx, int64_t n_items, bool approx) {
     static int per_sm[2] = {0, 0};
     if (!per_sm[0]) {
-        const void *k[2] = {(const void *)search_reads_kernel<S_COUNT>, (const void *)search_reads_kernel<S_ALL>};
-        for (int i = 0; i < 2; ++i) {
-            cudaFuncSetAttribute(k[i], cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-            int nb = 0;
-            if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k[i], RW * 32, 0) != cudaSuccess || nb < 1) nb = 1;
-            per_sm[i] = nb;
-        }
+        const void *k[2][2] = {{(const void *)search_reads_kernel<S_COUNT>, (const void *)search_reads_kernel<S_ALL>},
+                               {(const void *)search_reads_approx_kernel<S_COUNT>, (const void *)search_reads_approx_kernel<S_ALL>}};
+        for (int a = 0; a < 2; ++a)
+            for (int i = 0; i < 2; ++i) {
+                cudaFuncSetAttribute(k[a][i], cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+                int nb = 0;
+                if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k[a][i], RW * 32, 0) != cudaSuccess || nb < 1) nb = 1;
+                if (i == S_COUNT) per_sm[a] = nb;                   // the grid is sized by the count kernel
+            }
     }
     int64_t blocks = (n_items + RW - 1) / RW;
-    const int64_t maxb = (int64_t)ctx->sm_count * per_sm[0];
+    const int64_t maxb = (int64_t)ctx->sm_count * per_sm[approx ? 1 : 0];
     if (blocks > maxb) blocks = maxb;
     return blocks < 1 ? 1 : (int)blocks;
 }
 
-extern "C" int fxg_search_reads_host(fxg_ctx *ctx, const fxg_file *f, const fxg_fastq_row *d_rows, int64_t n_rows,
-                                     const uint8_t *pattern, int32_t m, int strands, fxg_search_hit **out, int64_t *n_out) {
+// fxg_search_reads_host (K8's exact test) and fxg_search_reads_approx_host (approx: at most max_mm mismatches)
+static int search_reads_host(fxg_ctx *ctx, const fxg_file *f, const fxg_fastq_row *d_rows, int64_t n_rows,
+                             const uint8_t *pattern, int32_t m, bool approx, int32_t max_mm, int strands, fxg_search_hit **out,
+                             int64_t *n_out) {
     if (!ctx && fxg_device_count() == 0) {
         fxg_set_error("no CUDA device available; libfxg has no CPU fallback");
         return FXG_ENODEV;
     }
     FXG_CHECK_ARG(ctx && f && out && n_out && pattern && n_rows >= 0, "bad arguments");
     FXG_CHECK_ARG(m >= 1 && m <= FXG_SEARCH_MAX_PATTERN, "pattern length must be 1 .. FXG_SEARCH_MAX_PATTERN");
+    FXG_CHECK_ARG(!approx || (max_mm >= 0 && max_mm < m), "max_mismatches must be 0 .. m - 1");
     FXG_CHECK_ARG(strands >= 1 && strands <= 3, "strands must be FXG_SEARCH_PLUS, FXG_SEARCH_MINUS or both");
     FXG_CHECK_ARG(n_rows == 0 || d_rows, "d_rows == NULL");
     *out = nullptr;
@@ -724,15 +794,17 @@ extern "C" int fxg_search_reads_host(fxg_ctx *ctx, const fxg_file *f, const fxg_
         A.tot = (int64_t *)ctx->search.ptr;
         int64_t *d_zero2 = A.tot + n_items, *d_hoff = d_zero2 + n_items;
         A.hit_off = d_hoff;
-        const int grid = search_reads_grid(ctx, n_items);
+        const int grid = search_reads_grid(ctx, n_items, approx);
         {
             FxgProfScope prof(ctx, FXG_PROF_GATHER);
-            search_reads_kernel<S_COUNT><<<grid, RW * 32, 0, ctx->stream>>>(A);
+            if (!approx) search_reads_kernel<S_COUNT><<<grid, RW * 32, 0, ctx->stream>>>(A);
+            else search_reads_approx_kernel<S_COUNT><<<grid, RW * 32, 0, ctx->stream>>>(A, max_mm);
         }
         FXG_CUDA(cudaGetLastError());
         rc = collect_hits(ctx, n_items, A.tot, d_zero2, d_hoff, [&](fxg_search_hit *o) {
             A.out = o;
-            search_reads_kernel<S_ALL><<<grid, RW * 32, 0, ctx->stream>>>(A);
+            if (!approx) search_reads_kernel<S_ALL><<<grid, RW * 32, 0, ctx->stream>>>(A);
+            else search_reads_approx_kernel<S_ALL><<<grid, RW * 32, 0, ctx->stream>>>(A, max_mm);
         }, &h, &n_hits);
         if (rc) return rc;
     }
@@ -743,4 +815,15 @@ extern "C" int fxg_search_reads_host(fxg_ctx *ctx, const fxg_file *f, const fxg_
     *out = h;
     *n_out = n_hits;
     return FXG_OK;
+}
+
+extern "C" int fxg_search_reads_host(fxg_ctx *ctx, const fxg_file *f, const fxg_fastq_row *d_rows, int64_t n_rows,
+                                     const uint8_t *pattern, int32_t m, int strands, fxg_search_hit **out, int64_t *n_out) {
+    return search_reads_host(ctx, f, d_rows, n_rows, pattern, m, false, 0, strands, out, n_out);
+}
+
+extern "C" int fxg_search_reads_approx_host(fxg_ctx *ctx, const fxg_file *f, const fxg_fastq_row *d_rows, int64_t n_rows,
+                                            const uint8_t *pattern, int32_t m, int32_t max_mismatches, int strands,
+                                            fxg_search_hit **out, int64_t *n_out) {
+    return search_reads_host(ctx, f, d_rows, n_rows, pattern, m, true, max_mismatches, strands, out, n_out);
 }

@@ -387,19 +387,36 @@ class Engine:
         them -- or, with row_id = s = e = None, in every whole record.  -> SEARCH_HIT array of (query, start, minus) in
         (query, start, minus) order, start relative to s; first=True keeps the first hit of each (query, strand)."""
         pat = bytes(pattern)
-        if row_id is None:
-            nq, rp, sp, ep = drows.n_rows, None, None, None
-        else:
-            row_id = np.ascontiguousarray(row_id, dtype=np.int64)
-            s = np.ascontiguousarray(s, dtype=np.int64)
-            e = np.ascontiguousarray(e, dtype=np.int64)
-            nq, rp, sp, ep = row_id.size, ptr(row_id), ptr(s), ptr(e)
+        nq, rp, sp, ep, keep = self._queries(drows, row_id, s, e)
         out = C.c_void_p()
         n = C.c_int64(0)
         check(lib().fxg_search_host(self.ctx, dfile.handle, drows.devptr, drows.n_rows, rp, sp, ep, int(flags), nq,
                                     pat, len(pat), int(strands), _cabi.SEARCH_FIRST if first else _cabi.SEARCH_ALL,
                                     C.byref(out), C.byref(n)))
         return self._take_hits(out, n)
+
+    def search_approx(self, dfile, drows, row_id, s, e, flags, pattern, max_mismatches, strands=_cabi.SEARCH_PLUS):
+        """Search with mismatches: every start of the queries' haystacks (as for search) within max_mismatches
+        substitutions of the pattern (or of its reverse complement on the minus strand).  -> SEARCH_HIT array of
+        (query, start, minus, mismatches) in (query, start, minus) order, start relative to s."""
+        pat = bytes(pattern)
+        nq, rp, sp, ep, keep = self._queries(drows, row_id, s, e)
+        out = C.c_void_p()
+        n = C.c_int64(0)
+        check(lib().fxg_search_approx_host(self.ctx, dfile.handle, drows.devptr, drows.n_rows, rp, sp, ep, int(flags),
+                                           nq, pat, len(pat), int(max_mismatches), int(strands), C.byref(out),
+                                           C.byref(n)))
+        return self._take_hits(out, n, with_mismatches=True)
+
+    @staticmethod
+    def _queries(drows, row_id, s, e):
+        """(nq, row_id, s, e pointers, the arrays they point into) of a search's queries; None: every whole record"""
+        if row_id is None:
+            return drows.n_rows, None, None, None, None
+        row_id = np.ascontiguousarray(row_id, dtype=np.int64)
+        s = np.ascontiguousarray(s, dtype=np.int64)
+        e = np.ascontiguousarray(e, dtype=np.int64)
+        return row_id.size, ptr(row_id), ptr(s), ptr(e), (row_id, s, e)
 
     def search_reads(self, dfile, drows, pattern, strands=_cabi.SEARCH_PLUS):
         """Exact pattern search (K8 on reads) in every FASTQ read of drows; a read's haystack is its raw sequence line
@@ -411,13 +428,24 @@ class Engine:
                                           C.byref(out), C.byref(n)))
         return self._take_hits(out, n)
 
+    def search_reads_approx(self, dfile, drows, pattern, max_mismatches, strands=_cabi.SEARCH_PLUS):
+        """Search with mismatches in every FASTQ read of drows (haystacks as for search_reads): every start within
+        max_mismatches substitutions.  -> SEARCH_HIT array of (query = read index, start, minus, mismatches) in
+        (query, start, minus) order."""
+        pat = bytes(pattern)
+        out = C.c_void_p()
+        n = C.c_int64(0)
+        check(lib().fxg_search_reads_approx_host(self.ctx, dfile.handle, drows.devptr, drows.n_rows, pat, len(pat),
+                                                 int(max_mismatches), int(strands), C.byref(out), C.byref(n)))
+        return self._take_hits(out, n, with_mismatches=True)
+
     @staticmethod
-    def _take_hits(out, n):
+    def _take_hits(out, n, with_mismatches=False):
         hits = np.zeros(n.value, dtype=_cabi.SEARCH_HIT)
         if n.value:
             C.memmove(hits.ctypes.data, out.value, n.value * _cabi.SEARCH_HIT.itemsize)
         lib().fxg_free_host(out)
-        return hits[["query", "start", "minus"]]
+        return hits if with_mismatches else hits[["query", "start", "minus"]]
 
     def read_one(self, dfile, drows, read_id, rlen, which=0, flags=0):
         """sequence (which = 0) or quality (1) bytes of one read: one kernel launch, one synchronisation"""

@@ -2,7 +2,7 @@
 """Time pattern search (K8) on the GPU, after verifying what it returns.
 
     python tools/time_search.py [--steps 10] [--warmup 2] [--records 1000000] [--big-mb 250] [--reads 126000000]
-                                [--sections locate,search,reads] [--profile] [--out FILE]
+                                [--sections locate,search,reads,approx] [--profile] [--out FILE]
 
 Inputs are generated in HBM with fxg_synth_fasta_dev / fxg_synth_fastq_dev:
     c2   the bench's C2 shape: 1 M FASTA records of U[9000, 11000] bp at 80 columns (~10.2 GB)
@@ -20,6 +20,14 @@ synchronisation, divided by `steps`):
               reads through fxg_search_host.  fraction_of_byte_floor: the time to move the 32-byte sectors covering
               every read's sequence plus 32 B per row at 3.35 TB/s, over the call time.  --profile: instead of the
               timings, torch.profiler device time of the new kernels (plan, count, emit)
+    approx    the search with mismatches (what Fasta.locate_approx and Fastq.locate_approx run) of the rare 12-mer at
+              k = 1, 2, 3 on "+" and "both", on C2 and on C4, alternating in the same call with the exact search of the
+              same pattern; ratio_to_exact is its time over the exact search's.  --profile: instead of the timings,
+              torch.profiler device time of the count and emit kernels and of the hit copy for each k on "+"
+
+Approx: every reported hit's window (through fxg_extract_host on C2, fxg_reads_host on C4) has the reported number of
+mismatches, at most k, against the pattern or its reverse complement; the per-record hit counts of the first 2,000 C2
+records and of the first 200,000 C4 reads equal those of numpy windows over the oracle's haystacks of the same bytes.
 
 Reads: every reported hit's window, fetched with fxg_reads_host, equals the pattern (or its reverse complement), and
 the per-read hit counts of the first 200,000 reads equal host bytes.find counts on those reads' bytes.
@@ -45,6 +53,7 @@ RARE = b"ACGTTGCATGCA"
 ECORI = b"GAATTC"
 N_ORACLE = 20000
 N_ORACLE_READS = 200000
+N_ORACLE_APPROX = 2000
 
 
 def gpu_info():
@@ -156,18 +165,122 @@ def verify_reads(eng, f, rows, pat, hits):
     return int(exp.sum())
 
 
+def make_fastq(eng, n):
+    """C4-shaped reads generated in HBM and scanned: (file, rows, device rows)"""
+    from pyfastx_b200 import _cabi
+    f = eng.alloc_file(n * (5 + 11 + 1 + 150 + 1 + 2 + 150 + 1) + digits_upto(n))
+    _cabi.check(_cabi.lib().fxg_synth_fastq_dev(eng.ctx, 20240602, n, 0, 150, None, f.devptr))
+    eng.sync()
+    rows, st, drows = eng.fastq_scan(f, keep_device_rows=True)
+    assert len(rows) == n
+    return f, rows, st, drows
+
+
+def window_counts(hay, pat):
+    """mismatches of every window of hay (uint8) against pat (uint8); rows of a 2-d hay are haystacks of their own"""
+    from numpy.lib.stride_tricks import sliding_window_view
+    return (sliding_window_view(hay, pat.size, axis=-1) != pat).sum(axis=-1)
+
+
+def verify_approx(windows, hay_counts, pat, k, hits, n_first):
+    """windows: the hits' windows (n_hits x m); hay_counts(p): per-window mismatch counts of the first n_first haystacks
+    against p, as a list of arrays -> number of hits checked against the oracle"""
+    from oracle import fxo
+    p = np.frombuffer(pat, np.uint8)
+    rc = fxo.complement_lut()[p][::-1]
+    q, mi, mm = hits["query"], hits["minus"].astype(bool), hits["mismatches"]
+    if q.size:
+        got = (windows != np.where(mi[:, None], rc[None, :], p[None, :])).sum(axis=1)
+        assert np.array_equal(got, mm) and int(mm.max()) <= k, "a reported hit's window has another mismatch count"
+    exp = np.zeros((n_first, 2), dtype=np.int64)
+    for s, pp in ((0, p), (1, rc)):
+        exp[:, s] = [int((c <= k).sum()) for c in hay_counts(pp)]
+    sel = q < n_first
+    got = np.zeros((n_first, 2), dtype=np.int64)
+    np.add.at(got, (q[sel], mi[sel].astype(np.int64)), 1)
+    assert np.array_equal(got, exp), "hit counts of the first haystacks differ from numpy windows over the oracle's"
+    return int(exp.sum())
+
+
+def section_approx(a, eng, stream, res):
+    """locate_approx of the rare 12-mer on C2 and C4, alternating with the exact search of the same pattern"""
+    import torch
+    from oracle import fxo
+    from pyfastx_b200 import _cabi, synth
+    both = _cabi.SEARCH_PLUS | _cabi.SEARCH_MINUS
+    out = res["approx"] = {"pattern": RARE.decode()}
+    for shape in ("c2", "c4"):
+        _cabi.lib().fxg_pool_trim()
+        if shape == "c2":
+            lengths = synth.fasta_lengths(a.records, 20240601, 9000, 11000)
+            f, off = make_fasta(eng, lengths)
+            rows, st, drows = eng.fasta_scan(f, keep_device_rows=True)
+            n_first = min(N_ORACLE_APPROX, len(rows))
+            head = f.download(0, int(off[n_first]))
+            orows, _, _ = fxo.fasta_scan(head)
+            hay, hoff, _ = fxo.subseq_batch(head, orows, np.arange(n_first), np.zeros(n_first, np.int64), orows["slen"],
+                                            np.zeros(n_first, np.int32))
+            hays = [hay[hoff[i]:hoff[i + 1]] for i in range(n_first)]
+            hay_counts = lambda p: [window_counts(h, p) for h in hays]
+            exact = lambda mask: eng.search(f, drows, None, None, None, 0, RARE, mask)
+            approx = lambda k, mask: eng.search_approx(f, drows, None, None, None, 0, RARE, k, mask)
+            def windows(h):
+                w, _, _ = eng.extract(f, drows, h["query"], h["start"], h["start"] + len(RARE), np.zeros(h.size, np.int32))
+                return w.reshape(-1, len(RARE))
+        else:
+            f, rows, st, drows = make_fastq(eng, a.reads)
+            n_first = min(N_ORACLE_READS, len(rows))
+            hb = f.download(0, int(rows["qoff"][n_first - 1] + rows["rlen"][n_first - 1] + 1))
+            orows, _, _ = fxo.fastq_scan(hb.tobytes())
+            assert len(orows) == n_first and np.all(orows["rlen"] == 150)
+            reads = hb[orows["soff"][:, None] + np.arange(150)[None, :]]
+            hay_counts = lambda p: list(window_counts(reads, p))
+            exact = lambda mask: eng.search_reads(f, drows, RARE, mask)
+            approx = lambda k, mask: eng.search_reads_approx(f, drows, RARE, k, mask)
+            def windows(h):
+                w, _ = eng.gather_ranges(f, rows["soff"][h["query"]] + h["start"], np.full(h.size, len(RARE), np.int64))
+                return w.reshape(-1, len(RARE))
+        o = out[shape] = {"file_gb": f.size / 1e9, "haystacks": len(rows), "bases": int(st["total_len"])}
+        for k in (1, 2, 3):
+            hits = approx(k, both)
+            o["k=%d oracle_checked_hits_first_%d" % (k, n_first)] = verify_approx(windows(hits), hay_counts, RARE, k,
+                                                                                 hits, n_first)
+            del hits
+        if a.profile:
+            from torch.profiler import ProfilerActivity, profile
+            prof_out = o["profile_plus"] = {}
+            for k in (1, 2, 3):
+                approx(k, _cabi.SEARCH_PLUS)
+                with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                    approx(k, _cabi.SEARCH_PLUS)
+                    torch.cuda.synchronize()
+                prof_out["k=%d" % k] = {ev.key: {"calls": ev.count, "device_ms_total": round(ev.device_time_total / 1e3, 3)}
+                                        for ev in prof.key_averages() if "approx" in ev.key or "Memcpy DtoH" in ev.key}
+        else:
+            for k in (1, 2, 3):
+                for strand, mask in (("+", _cabi.SEARCH_PLUS), ("both", both)):
+                    new, old = (lambda: approx(k, mask)), (lambda: exact(mask))
+                    for _ in range(a.warmup):
+                        new(); old()
+                    n_hits = len(new())
+                    tn, to = [], []
+                    for _ in range(3):                              # alternating, in the same call
+                        tn.append(timed(stream, a.steps, new))
+                        to.append(timed(stream, a.steps, old))
+                    med, medo = float(np.median(tn)), float(np.median(to))
+                    o["k=%d %s" % (k, strand)] = {
+                        "hits": n_hits, "ms_median": round(med, 3), "ms_min": round(min(tn), 3), "ms_max": round(max(tn), 3),
+                        "exact_ms_median": round(medo, 3), "ratio_to_exact": round(med / medo, 2)}
+        drows.free(); f.free()
+
+
 def section_reads(a, eng, stream, res):
     """Fastq.locate's call on the C4 shape, against the stand-in route: one-line FASTA rows over the same reads
     through fxg_search_host"""
     import torch
     from pyfastx_b200 import _cabi
-    L = _cabi.lib()
     n = a.reads
-    f = eng.alloc_file(n * (5 + 11 + 1 + 150 + 1 + 2 + 150 + 1) + digits_upto(n))
-    _cabi.check(L.fxg_synth_fastq_dev(eng.ctx, 20240602, n, 0, 150, None, f.devptr))
-    eng.sync()
-    rows, st, drows = eng.fastq_scan(f, keep_device_rows=True)
-    assert len(rows) == n
+    f, rows, st, drows = make_fastq(eng, n)
     # bytes the search has to read at the least: the 32-byte sectors covering every read's sequence, and its row
     soff, rlen = rows["soff"], rows["rlen"]
     floor = int(((((soff + rlen + 31) >> 5) - (soff >> 5)) * 32).sum()) + 32 * n
@@ -237,7 +350,10 @@ def main():
     res = {"gpu": gpu_info(), "device": torch.cuda.get_device_name(0), "locate": {}, "search": {}}
     sections = a.sections.split(",")
     if a.profile:
-        section_reads(a, eng, stream, res)
+        if "reads" in sections:
+            section_reads(a, eng, stream, res)
+        if "approx" in sections:
+            section_approx(a, eng, stream, res)
         sections = []
 
     if "locate" in sections:
@@ -300,6 +416,8 @@ def main():
     if "reads" in sections:
         _cabi.lib().fxg_pool_trim()                         # the freed C2 / big buffers stay pooled: give them back
         section_reads(a, eng, stream, res)
+    if "approx" in sections:
+        section_approx(a, eng, stream, res)
     s = json.dumps(res, indent=1)
     if a.out:
         with open(a.out, "w") as fh:
