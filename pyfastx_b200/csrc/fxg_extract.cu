@@ -74,22 +74,15 @@ __device__ void gather_one(const uint8_t *__restrict__ file, int64_t fsize, cons
         uint32_t valid = 0;                                      // combined-mask bits of in-range bytes
         if (my < src_end && my + 16 > job.src) {
             v = *reinterpret_cast<const uint4 *>(file + my);
-            int lo = (int)(job.src > my ? job.src - my : 0);
-            int hi = (int)(src_end - my < 16 ? src_end - my : 16);
-            // mask with bytes lo..hi-1
+            const int lo = (int)(job.src > my ? job.src - my : 0);
+            const int hi = (int)(src_end - my < 16 ? src_end - my : 16);
+            // combined-mask bits of bytes lo..hi-1, byte by byte: no byte at or past hi may count, or a range holding
+            // fewer kept bytes than requested would take the kept byte after its end instead of the zero fill below
+            // (test_edge_layouts_gpu.py::test_slice_short_of_kept_bytes)
             uint32_t m = 0;
 #pragma unroll
-            for (int w = 0; w < 4; ++w) {
-                // bytes 4w..4w+3 -> combined bits (8b + 7 - w)
-                int l = lo - 4 * w, h = hi - 4 * w;
-                l = l < 0 ? 0 : (l > 4 ? 4 : l);
-                h = h < 0 ? 0 : (h > 4 ? 4 : h);
-                if (h > l) {
-                    uint32_t word_bits = ((h == 4 ? 0xffffffffu : ((1u << (8 * h)) - 1u)) & ~((1u << (8 * l)) - 1u)) & 0x80808080u;
-                    if (l == 0 && h == 4) word_bits = 0x80808080u;
-                    m |= word_bits >> w;
-                }
-            }
+            for (int off = 0; off < 16; ++off)
+                if (off >= lo && off < hi) m |= bit_of_off(off);
             valid = m;
         }
         uint32_t keep = raw ? valid : (valid & ~keep_mask16(v));
