@@ -148,7 +148,10 @@ void        fxg_host_free(void *p);
 /* ---- file staging: raw bytes -> HBM ------------------------------------------------------
  * Replaces the reference's read side: gzread into a 1 MiB kstream buffer (src/kseq.c:70)
  * for the scan, fseeko+fread per request for random access (src/index.c:683-692,
- * src/read.c:37-45).  The whole file becomes one padded device buffer. */
+ * src/read.c:37-45).  The whole file becomes one padded device buffer.
+ * fxg_file_alloc (its padding), fxg_file_upload, fxg_file_from_host and fxg_file_slice return with their copies
+ * complete, like fxg_file_from_path: the single-query calls (fxg_extract_one_host, fxg_read_one_host) may be served
+ * from a stream of the library's own that does not wait for the context's stream. */
 int      fxg_file_alloc(fxg_ctx *ctx, int64_t nbytes, fxg_file **out);
 int      fxg_file_upload(fxg_ctx *ctx, fxg_file *f, int64_t dst_off, const void *host, int64_t nbytes);
 int      fxg_file_from_host(fxg_ctx *ctx, const void *host, int64_t nbytes, fxg_file **out);

@@ -191,9 +191,22 @@ void fxg_pool_drain(int device) {
 }
 extern "C" void fxg_pool_trim(void) { fxg_pool_drain(-1); }
 
-extern "C" int fxg_file_alloc(fxg_ctx *c, int64_t nbytes, fxg_file **out) {
-    FXG_CHECK_ARG(c && out && nbytes >= 0, "bad arguments");
-    FXG_LOCK(c);
+// The public staging entry points (fxg_file_alloc / _upload / _from_host / _slice) return with their copies complete:
+// the single-query service reads file buffers from a stream of its own, which does not wait for the context's stream.
+// fxg_file_alloc_async / fxg_file_upload_async only enqueue; library calls that synchronise before they return anyway
+// (the path stager, the one-call index builds, the GPU inflate paths) use them directly.
+static int file_done(fxg_ctx *c, fxg_file **out, int rc) {
+    if (rc == FXG_OK) {
+        const cudaError_t e = cudaStreamSynchronize(c->stream);
+        if (e == cudaSuccess) return FXG_OK;
+        fxg_set_error("file staging failed: %s", cudaGetErrorString(e));
+        rc = FXG_ECUDA;
+    }
+    if (out && *out) { fxg_file_free(*out); *out = nullptr; }
+    return rc;
+}
+
+int fxg_file_alloc_async(fxg_ctx *c, int64_t nbytes, fxg_file **out) {
     *out = nullptr;
     FXG_CUDA(cudaSetDevice(c->device));
     fxg_file *f = new fxg_file();
@@ -229,9 +242,15 @@ extern "C" int fxg_file_alloc(fxg_ctx *c, int64_t nbytes, fxg_file **out) {
     }
     // zero the padding (never contains '\n'); data region is overwritten by uploads
     const int64_t pad_from = nbytes & ~(int64_t)15;
-    FXG_CUDA(cudaMemsetAsync(f->d + pad_from, 0, (size_t)(f->capacity - pad_from), c->stream));
     *out = f;
+    FXG_CUDA(cudaMemsetAsync(f->d + pad_from, 0, (size_t)(f->capacity - pad_from), c->stream));
     return FXG_OK;
+}
+
+extern "C" int fxg_file_alloc(fxg_ctx *c, int64_t nbytes, fxg_file **out) {
+    FXG_CHECK_ARG(c && out && nbytes >= 0, "bad arguments");
+    FXG_LOCK(c);
+    return file_done(c, out, fxg_file_alloc_async(c, nbytes, out));
 }
 
 static bool host_ptr_is_pinned(const void *p) {
@@ -268,9 +287,7 @@ static void parallel_memcpy(void *dst, const void *src, size_t n) {
     for (auto &t : th) t.join();
 }
 
-extern "C" int fxg_file_upload(fxg_ctx *c, fxg_file *f, int64_t dst_off, const void *host, int64_t nbytes) {
-    FXG_CHECK_ARG(c && f && (host || nbytes == 0), "bad arguments");
-    FXG_LOCK(c);
+int fxg_file_upload_async(fxg_ctx *c, fxg_file *f, int64_t dst_off, const void *host, int64_t nbytes) {
     FXG_CHECK_ARG(dst_off >= 0 && nbytes >= 0 && dst_off + nbytes <= f->size, "upload range outside file");
     FXG_CUDA(cudaSetDevice(c->device));
     if (nbytes == 0) return FXG_OK;
@@ -297,14 +314,18 @@ extern "C" int fxg_file_upload(fxg_ctx *c, fxg_file *f, int64_t dst_off, const v
     return FXG_OK;
 }
 
-extern "C" int fxg_file_from_host(fxg_ctx *c, const void *host, int64_t nbytes, fxg_file **out) {
-    if (!c) { fxg_set_error("invalid argument: ctx == NULL"); return FXG_EINVAL; }
+extern "C" int fxg_file_upload(fxg_ctx *c, fxg_file *f, int64_t dst_off, const void *host, int64_t nbytes) {
+    FXG_CHECK_ARG(c && f && (host || nbytes == 0), "bad arguments");
     FXG_LOCK(c);
-    int rc = fxg_file_alloc(c, nbytes, out);
-    if (rc) return rc;
-    rc = fxg_file_upload(c, *out, 0, host, nbytes);
-    if (rc) { fxg_file_free(*out); *out = nullptr; }
-    return rc;
+    return file_done(c, nullptr, fxg_file_upload_async(c, f, dst_off, host, nbytes));
+}
+
+extern "C" int fxg_file_from_host(fxg_ctx *c, const void *host, int64_t nbytes, fxg_file **out) {
+    FXG_CHECK_ARG(c && out && nbytes >= 0 && (host || nbytes == 0), "bad arguments");
+    FXG_LOCK(c);
+    int rc = fxg_file_alloc_async(c, nbytes, out);
+    if (rc == FXG_OK) rc = fxg_file_upload_async(c, *out, 0, host, nbytes);
+    return file_done(c, out, rc);
 }
 
 // NUMA node that holds the page-cache pages of bytes [begin, end) of an open file (sampled at three offsets), -1 if unknown.
@@ -370,8 +391,8 @@ static int stage_path_range(fxg_ctx *c, const char *path, int64_t begin, int64_t
     if (end < 0 || end > (int64_t)st.st_size) end = (int64_t)st.st_size;
     if (begin > end) begin = end;
     const int64_t n = end - begin;
-    int rc = fxg_file_alloc(c, n, out);
-    if (rc) { close(fd); return rc; }
+    int rc = fxg_file_alloc_async(c, n, out);                           // the stream is synchronised below
+    if (rc) { close(fd); if (*out) { fxg_file_free(*out); *out = nullptr; } return rc; }
     if (!c->ring) {
         cudaError_t e = cudaHostAlloc(&c->ring, (size_t)(RING_PIECE * RING_SLOTS), cudaHostAllocDefault);
         if (e != cudaSuccess) { cudaGetLastError(); c->ring = nullptr; close(fd); fxg_file_free(*out); *out = nullptr; fxg_set_error("cudaHostAlloc of the staging ring failed: %s", cudaGetErrorString(e)); return FXG_ENOMEM; }
@@ -465,11 +486,12 @@ extern "C" int fxg_file_from_path_range(fxg_ctx *c, const char *path, int64_t be
 extern "C" int fxg_file_slice(fxg_ctx *c, const fxg_file *src, int64_t begin, int64_t end, fxg_file **out) {
     FXG_CHECK_ARG(c && src && out && begin >= 0 && end >= begin && end <= src->size, "bad arguments");
     FXG_LOCK(c);
-    int rc = fxg_file_alloc(c, end - begin, out);
-    if (rc) return rc;
-    if (end > begin)
-        FXG_CUDA(cudaMemcpyAsync((*out)->d, src->d + begin, (size_t)(end - begin), cudaMemcpyDeviceToDevice, c->stream));
-    return FXG_OK;
+    int rc = fxg_file_alloc_async(c, end - begin, out);
+    if (rc == FXG_OK && end > begin) {
+        const cudaError_t e = cudaMemcpyAsync((*out)->d, src->d + begin, (size_t)(end - begin), cudaMemcpyDeviceToDevice, c->stream);
+        if (e != cudaSuccess) { fxg_set_error("device copy failed: %s", cudaGetErrorString(e)); rc = FXG_ECUDA; }
+    }
+    return file_done(c, out, rc);
 }
 
 // Split point on a host file (SURVEY.md section 8e): first offset >= from where a line (or a FASTA header line,
@@ -597,7 +619,7 @@ static int stage_into_ctx(fxg_ctx *c, const void *host_buf, int64_t nbytes, fxg_
     view->size = nbytes; view->capacity = cap; view->owned = false; view->device = c->device;
     const int64_t pad_from = nbytes & ~(int64_t)15;
     FXG_CUDA(cudaMemsetAsync(view->d + pad_from, 0, (size_t)(cap - pad_from), c->stream));
-    return fxg_file_upload(c, view, 0, host_buf, nbytes);
+    return fxg_file_upload_async(c, view, 0, host_buf, nbytes);        // the build synchronises before it returns
 }
 
 extern "C" int fxg_fasta_build_index_host(fxg_ctx *c, const void *host_buf, int64_t nbytes, int flags,

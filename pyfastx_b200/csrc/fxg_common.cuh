@@ -11,6 +11,10 @@
 // host side
 // ---------------------------------------------------------------------------------------
 void fxg_set_error(const char *fmt, ...);
+// fxg_file_alloc / fxg_file_upload without their closing stream synchronisation (fxg_api.cu), for library calls that
+// synchronise the context's stream before they return
+int fxg_file_alloc_async(fxg_ctx *c, int64_t nbytes, fxg_file **out);
+int fxg_file_upload_async(fxg_ctx *c, fxg_file *f, int64_t dst_off, const void *host, int64_t nbytes);
 
 #define FXG_CUDA(call)                                                                    \
     do {                                                                                  \

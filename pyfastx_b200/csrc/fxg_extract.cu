@@ -1304,7 +1304,9 @@ static bool svc_enabled() {
     if (on < 0) { const char *e = getenv("FXG_ONE_SERVICE"); on = (e && e[0] == '0') ? 0 : 1; }
     return on != 0;
 }
-void fxg_svc_stop(fxg_ctx *ctx) {                       // called by fxg_ctx_destroy and before buffers a query may name are freed
+// Called by fxg_ctx_destroy.  Freeing a buffer that a query named needs no stop: cudaFree, and the file pool's
+// cudaDeviceSynchronize before it hands a buffer on, wait for the resident kernel, which leaves after its idle period.
+void fxg_svc_stop(fxg_ctx *ctx) {
     if (!ctx->svc_req) return;
     OneRequest *rq = (OneRequest *)ctx->svc_req;
     ((volatile OneRequest *)rq)->stop = 1;
@@ -1336,7 +1338,8 @@ static int svc_query(fxg_ctx *ctx, const fxg_file *f, const void *d_rows_any, in
         ctx->svc_next = 1;
     }
     // results of earlier work on the context's stream (staging, scan, row uploads) must be complete: every host entry point
-    // that produces them synchronises before it returns, so there is nothing to wait for here
+    // that produces them synchronises before it returns (the file staging calls too, include/fxg.h), so there is nothing
+    // to wait for here
     volatile OneRequest *rq = (volatile OneRequest *)ctx->svc_req;
     const unsigned long long n = ctx->svc_next;
     // second half first, `tail` last; then the first half, `head` last (x86 keeps the store order)

@@ -248,8 +248,9 @@ extern "C" int fxg_file_from_bgzf_host(fxg_ctx *ctx, const void *host_buf, int64
     void *d_tab = nullptr;
     int32_t *d_status = nullptr;
     int32_t *h_status = nullptr;
-    if (!rc) rc = fxg_file_from_host(ctx, host_buf, nbytes, &cf);
-    if (!rc) rc = fxg_file_alloc(ctx, total, &uf);
+    if (!rc) rc = fxg_file_alloc_async(ctx, nbytes, &cf);           // the stream is synchronised below
+    if (!rc) rc = fxg_file_upload_async(ctx, cf, 0, host_buf, nbytes);
+    if (!rc) rc = fxg_file_alloc_async(ctx, total, &uf);
     if (!rc) rc = fxg_rows_upload(ctx, tab, (n + 1) * 2, (int)sizeof(int64_t), &d_tab);
     if (!rc && cudaMalloc((void **)&d_status, (size_t)(n + 1) * sizeof(int32_t)) != cudaSuccess) { fxg_set_error("cudaMalloc failed"); rc = FXG_ENOMEM; }
     if (!rc) rc = fxg_inflate_members_dev(ctx, cf, (const int64_t *)d_tab, (const int64_t *)d_tab + n + 1, n, uf->d, total, d_status);
@@ -309,8 +310,9 @@ extern "C" int fxg_file_from_gzip_points_host(fxg_ctx *ctx, const void *host_buf
     uint32_t *d_crc = nullptr;
     std::vector<int32_t> h_status((size_t)n);
     std::vector<uint32_t> h_crc((size_t)n);
-    int rc = fxg_file_from_host(ctx, host_buf, nbytes, &cf);
-    if (!rc) rc = fxg_file_alloc(ctx, total, &uf);
+    int rc = fxg_file_alloc_async(ctx, nbytes, &cf);                // the stream is synchronised below
+    if (!rc) rc = fxg_file_upload_async(ctx, cf, 0, host_buf, nbytes);
+    if (!rc) rc = fxg_file_alloc_async(ctx, total, &uf);
     if (!rc) rc = fxg_rows_upload(ctx, gz->cmp_offset, n, 8, &d_co);
     if (!rc) rc = fxg_rows_upload(ctx, uo.data(), n + 1, 8, &d_uo);
     if (!rc) rc = fxg_rows_upload(ctx, bt.data(), n, 1, &d_bt);

@@ -230,19 +230,18 @@ def test_compiled_object_layer_keys_and_fastx(tmp_path):
         assert recs[q["id"]][1] == q["seq"] and recs[q["id"]][2] == q["qual"] and recs[q["id"]][0] == fq[q["id"]].name
 
 
-@pytest.mark.gpu
-@pytest.mark.parametrize("service", ["1", "0"])
-def test_per_object_getters_service_and_launch_paths(tmp_path, monkeypatch, service):
-    """fa[name][s:e].seq / .antisense and fq[i].seq / .qual one query per call -- through the resident service kernel
-    (mapped-memory requests, no launch per query) and through the launch + synchronise path: identical to the batched
-    API, also after the service kernel has left on its idle period (sleep) and for queries that span several warps"""
+def _getters_body(tmp):
+    """fa[name][s:e].seq / .antisense and fq[i].seq / .qual / .antisense one query per call against the batched API,
+    with a sleep past the service kernel's idle period halfway -> (getter calls, calls longer than the service takes,
+    launches the getter calls added)"""
     import time
-    monkeypatch.setenv("FXG_ONE_SERVICE", service)
     import pyfastx_b200
-    from pyfastx_b200 import synth
-    p = tmp_path / "s.fa"
-    p.write_bytes(synth.synth_fasta(60, seed=11))
-    fa = pyfastx_b200.Fasta(str(p))
+    from pyfastx_b200 import _cabi, synth
+    p = os.path.join(tmp, "s.fa")
+    with open(p, "wb") as fh:
+        fh.write(synth.synth_fasta(60, seed=11))
+    fa = pyfastx_b200.Fasta(p)
+    ctx = fa._st.engine.ctx
     rng = np.random.default_rng(5)
     names, qs, qe, minus = [], [], [], []
     for k in range(300):
@@ -253,21 +252,57 @@ def test_per_object_getters_service_and_launch_paths(tmp_path, monkeypatch, serv
         a = int(rng.integers(0, n - L + 1))
         names.append(fa[i].name); qs.append(a); qe.append(a + L); minus.append(bool(k & 1))
     want = fa.fetch_many(names, np.array(qs) + 1, np.array(qe), ["-" if m else "+" for m in minus])
+    calls, long_calls, launched = 0, 0, 0
     for k in range(300):
         sub = fa[names[k]][qs[k]:qe[k]]
-        assert (sub.antisense if minus[k] else sub.seq) == want[k], k
+        n0 = _cabi.lib().fxg_ctx_launch_count(ctx)
+        got = sub.antisense if minus[k] else sub.seq
+        launched += _cabi.lib().fxg_ctx_launch_count(ctx) - n0
+        calls += 1
+        long_calls += qe[k] - qs[k] > 65536
+        assert got == want[k], k
         if k == 150:
             time.sleep(0.02)                                  # longer than the service kernel's idle period: it relaunches
-    q = tmp_path / "s.fq"
-    q.write_bytes(synth.synth_fastq(500, seed=12))
-    fq = pyfastx_b200.Fastq(str(q))
+    q = os.path.join(tmp, "s.fq")
+    with open(q, "wb") as fh:
+        fh.write(synth.synth_fastq(500, seed=12))
+    fq = pyfastx_b200.Fastq(q)
     ids = [int(x) for x in rng.integers(0, len(fq), size=100)]
     sq, ql, off = fq.reads_many(ids)
+    want = []
+    for k in range(len(ids)):
+        want_seq = bytes(sq[off[k]:off[k + 1]]).decode()
+        want.append((want_seq, bytes(ql[off[k]:off[k + 1]]).decode(), pyfastx_b200.reverse_complement(want_seq)))
     for k, i in enumerate(ids):
         r = fq[i]
-        want_seq = bytes(sq[off[k]:off[k + 1]]).decode()
-        assert r.seq == want_seq and r.qual == bytes(ql[off[k]:off[k + 1]]).decode()
-        assert r.antisense == pyfastx_b200.reverse_complement(want_seq)
+        n0 = _cabi.lib().fxg_ctx_launch_count(ctx)
+        got = (r.seq, r.qual, r.antisense)
+        launched += _cabi.lib().fxg_ctx_launch_count(ctx) - n0
+        calls += 3
+        assert got == want[k], k
+    return calls, long_calls, launched
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("service", ["1", "0"])
+def test_per_object_getters_service_and_launch_paths(tmp_path, service):
+    """the per-object getters one query per call through the resident service kernel (mapped-memory requests, no
+    launch per query) and through the launch + synchronise path: identical to the batched API, also after the service
+    kernel has left on its idle period and for queries that span several warps.  The library reads FXG_ONE_SERVICE
+    once per process, so the launch path ("0") runs in a child process started with FXG_ONE_SERVICE=0."""
+    if service == "1":
+        calls, long_calls, launched = _getters_body(str(tmp_path))
+        assert launched <= long_calls + 4, (calls, long_calls, launched)      # plus the service kernel's (re)launches
+        return
+    import subprocess
+    code = ("import sys; sys.path[:0] = [%r, %r]; import test_api_gpu as T; print(*T._getters_body(%r))"
+            % (os.path.join(ROOT, "tests"), ROOT, str(tmp_path)))
+    cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + ["-c", code]
+    p = subprocess.run(cmd, env=dict(os.environ, FXG_ONE_SERVICE="0"), cwd=ROOT, capture_output=True, text=True,
+                       timeout=600)
+    assert p.returncode == 0, p.stdout[-3000:] + p.stderr[-3000:]
+    calls, long_calls, launched = (int(x) for x in p.stdout.split()[-3:])
+    assert calls == 600 and launched == calls, (calls, launched)               # one launch per getter call
 
 
 @pytest.mark.gpu
