@@ -97,18 +97,16 @@ FXI_HD int slow_decode(Bits &br, const uint16_t *cnt, const uint16_t *sym) {
     return -1;
 }
 
-// Primary + canonical tables for `n` symbols with code lengths lens[0..n).  False if over-subscribed.
+// Primary + canonical tables for `n` symbols with code lengths lens[0..n).  False, as zlib's inflate_table decides, if
+// the code is over-subscribed, or incomplete unless it is empty or a single code of length 1.
 FXI_HD bool build_table(const uint8_t *lens, int n, uint16_t *tab, int tab_bits, int sym_shift, uint16_t *cnt,
                         uint16_t *sym) {
     for (int i = 0; i < 16; ++i) cnt[i] = 0;
     for (int i = 0; i < n; ++i) cnt[lens[i]]++;
     int left = 1;
-    bool ok = true;
-    for (int len = 1; len <= 15; ++len) {
-        left <<= 1;
-        left -= cnt[len];
-        if (left < 0) ok = false;
-    }
+    for (int len = 1; len <= 15; ++len) left = (left << 1) - cnt[len];     // once negative, stays negative
+    // complete; or no code at all; or one code of length 1 (which alone leaves 2^14 of the 2^15 code space)
+    const bool ok = left == 0 || left == (1 << 15) || (left == (1 << 14) && cnt[1] == 1);
     uint16_t offs[16], next[16];
     offs[1] = 0;
     for (int len = 1; len < 15; ++len) offs[len + 1] = (uint16_t)(offs[len] + cnt[len]);
@@ -232,8 +230,11 @@ struct Decoder {
         br.pos = p;
     }
 
+    // A member's deflate data must end in the byte before its trailer: zlib reads the trailer right after the last
+    // block, so bytes in between fail its CRC check even when the trailer describes the output correctly.
     FXI_HD void finish_member() {
         if (status == INF_OK && opos != o1) status = INF_SIZE;
+        else if (status == INF_OK && !seg && br.pos - (br.nbits >> 3) != dend) status = INF_BAD_BLOCK;
         state = DONE;
     }
 
@@ -256,8 +257,8 @@ struct Decoder {
             return;                                           // still NEED_BLOCK (or the end, next step)
         } else if (btype == 1) {
             for (int i = 0; i < 288; ++i) lens[i] = (uint8_t)(i < 144 ? 8 : (i < 256 ? 9 : (i < 280 ? 7 : 8)));
-            for (int i = 0; i < 30; ++i) lens[288 + i] = 5;
-            hlit = 288; hdist = 30;
+            for (int i = 0; i < 32; ++i) lens[288 + i] = 5;      // all 32 codes: a complete code; 30 and 31 are rejected when read
+            hlit = 288; hdist = 32;
         } else if (btype == 2) {
             hlit = (int)br.get(5) + 257;
             hdist = (int)br.get(5) + 1;
@@ -266,7 +267,13 @@ struct Decoder {
             // code-length code: tiny canonical decoder, bit by bit
             uint8_t cl[19];
             for (int i = 0; i < 19; ++i) cl[i] = 0;
-            for (int i = 0; i < hclen; ++i) cl[K.CL_ORDER[i]] = (uint8_t)br.get(3);
+            int kraft = 0;                                   // code space the code-length code fills, of 128
+            for (int i = 0; i < hclen; ++i) {
+                const int v = (int)br.get(3);
+                cl[K.CL_ORDER[i]] = (uint8_t)v;
+                kraft += v ? 128 >> v : 0;
+            }
+            if (kraft != 128) { fail(INF_BAD_CODE); return; }   // complete, as zlib requires
             uint16_t ccnt[8], csym[19], offs[8];
             for (int i = 0; i < 8; ++i) ccnt[i] = 0;
             for (int i = 0; i < 19; ++i) ccnt[cl[i]]++;
@@ -299,7 +306,7 @@ struct Decoder {
         if (br.overrun()) { fail(INF_OVERRUN); return; }
         bool ok = build_table(lens, hlit, T.lit, TL_BITS, 9, T.litcnt, T.litsym);
         ok = build_table(lens + hlit, hdist, T.dist, TD_BITS, 5, T.distcnt, T.distsym) && ok;
-        // an incomplete distance code with a single symbol is legal; over-subscription is not
+        // over-subscribed or incomplete codes are invalid, except a single one-bit code and an empty distance code
         if (!ok) { fail(INF_BAD_CODE); return; }
         state = SYMBOLS;
     }
