@@ -110,12 +110,63 @@ struct FqStats {
     int minqs, maxqs;
 };
 
-// bytes of the line starting at `s` (to the next '\n' or the end of the file), 16 per lane and step
+// The reference's walk over a quality line of L bytes (src/fastq.c:732-745) shortens the line by one at each '\r' it
+// meets and skips it, so byte i is visited iff i + ('\r' before i) < L: a '\r' before the last byte ends the walk
+// early.  Exact form for the lines fq_line cannot settle in one pass (L known): -> the walk's length; the visited
+// bytes' range goes to mn / mx.
+__device__ __forceinline__ int64_t fq_qual_exact(const uint8_t *__restrict__ file, int64_t n, int64_t s, int64_t L, int lane,
+                                              int &mn, int &mx) {
+    int64_t carry = 0;                                                  // '\r' of the line before this step
+    int vis_cr = 0;
+    for (int64_t o0 = s & ~(int64_t)15; o0 < s + L; o0 += 512) {
+        const int64_t o = o0 + lane * 16;
+        uint4 v = make_uint4(0, 0, 0, 0);
+        if (o < n) v = *reinterpret_cast<const uint4 *>(file + o);
+        const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+        int c = 0;
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+            const uint32_t ch = (w[i >> 2] >> (8 * (i & 3))) & 0xffu;
+            c += (o + i >= s && o + i < s + L && ch == 13u);
+        }
+        int incl = c;                                                   // inclusive prefix over the lanes
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const int t = __shfl_up_sync(0xffffffffu, incl, d);
+            if (lane >= d) incl += t;
+        }
+        int64_t before = carry + incl - c;
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+            const int64_t p = o + i - s;
+            if (p >= 0 && p < L) {
+                const uint32_t ch = (w[i >> 2] >> (8 * (i & 3))) & 0xffu;
+                if (p + before < L) {
+                    if (ch == 13u) ++vis_cr;
+                    else {
+                        const int sc = (int)(signed char)ch;
+                        mn = sc < mn ? sc : mn;
+                        mx = sc > mx ? sc : mx;
+                    }
+                }
+                before += ch == 13u;
+            }
+        }
+        carry += __shfl_sync(0xffffffffu, incl, 31);
+    }
+    return L - __reduce_add_sync(0xffffffffu, vis_cr);
+}
+
+// bytes of the line starting at `s` (to the next '\n' or the end of the file), 16 per lane and step.  A sequence
+// line counts every byte but '\r'; a quality line gives the reference's length and quality range (fq_qual_exact):
+// settled in this pass when its only '\r' is the last byte or it has none, else by a second, exact pass.
 template <bool QUAL>
 __device__ __forceinline__ void fq_line(const uint8_t *__restrict__ file, int64_t n, int64_t s, int lane,
                                         uint32_t &cA, uint32_t &cC, uint32_t &cG, uint32_t &cT, uint32_t &cOther,
                                         int &mn, int &mx, int64_t &len_out) {
     int64_t len = 0;
+    int cr = 0;                                                           // QUAL: this lane's '\r' of the line
+    int lmn = 1 << 20, lmx = -(1 << 20);                                  // QUAL: range of the line's other bytes
     bool done = false;
     for (int64_t o0 = s & ~(int64_t)15; !done; o0 += 512) {
         const int64_t o = o0 + lane * 16;
@@ -145,13 +196,24 @@ __device__ __forceinline__ void fq_line(const uint8_t *__restrict__ file, int64_
                     else if (ch != 13u) ++cOther;
                 } else if (ch != 13u) {
                     const int sc = (int)(signed char)ch;                       // the reference compares plain (signed) chars
-                    mn = sc < mn ? sc : mn;
-                    mx = sc > mx ? sc : mx;
-                } else --got;                                                  // '\r' does not count towards the length
+                    lmn = sc < lmn ? sc : lmn;
+                    lmx = sc > lmx ? sc : lmx;
+                } else { --got; ++cr; }                                        // '\r' does not count towards the length
             }
         }
         len += __reduce_add_sync(0xffffffffu, got);
         done = has != 0 || o0 + 512 >= n;
+    }
+    if (QUAL) {
+        const int crs = __reduce_add_sync(0xffffffffu, cr);
+        const int64_t L = len + crs;                                         // bytes before the terminator
+        // no '\r', or one as the last byte (a CRLF line): every byte but the '\r' is visited
+        if (crs == 0 || (crs == 1 && file[s + L - 1] == 13u)) {
+            mn = lmn < mn ? lmn : mn;
+            mx = lmx > mx ? lmx : mx;
+        } else {
+            len = fq_qual_exact(file, n, s, L, lane, mn, mx);
+        }
     }
     len_out = len;
 }
