@@ -240,6 +240,8 @@ __device__ bool pull_one(const uint8_t *__restrict__ file, int64_t boff, int64_t
                     V[i] = (V[i] & ~m) | (e2 & m);
                 }
                 if (elen == 2 && file[p + c] != '\r') bad = true;      // the skipped byte must be strippable
+            } else if (c == (uint32_t)nb && elen == 2 && file[p + c] != '\r') {
+                bad = true;                                             // a break right after the word: checked here too
             }
             // valid-byte masks (0x80 per byte) of the first nb bytes
             uint32_t vb[4];
@@ -579,7 +581,8 @@ __global__ void __launch_bounds__(XTHREADS, 3) extract_bulk_kernel(
             if (t1 - d1 * bpl >= bpl) ++d1;
             uint32_t t2 = rem_s + rb1, d2 = __umulhi(t2, inv);
             if (t2 - d2 * bpl >= bpl) ++d2;
-            const int rel1 = (int)(ra + (uint32_t)elen * d1), rel2 = (int)(rb1 + (uint32_t)elen * d2) + 1;
+            // rel2 also covers the byte after the last kept one: the '\r' of a break that follows the item's last word
+            const int rel1 = (int)(ra + (uint32_t)elen * d1), rel2 = (int)(rb1 + (uint32_t)elen * d2) + (elen == 2 ? 2 : 1);
             const int fqa = (int)(reinterpret_cast<uintptr_t>(fq) & 15);
             g0 = rel1 - ((fqa + rel1) & 15);
             const int g1 = rel2 + ((16 - ((fqa + rel2) & 15)) & 15);
@@ -682,6 +685,9 @@ __global__ void __launch_bounds__(XTHREADS, 3) extract_bulk_kernel(
                             const uint32_t m = __funnelshift_lc(0u, 0xffffffffu, max(c8 - 32 * i, 0));
                             V[i] = (V[i] & ~m) | (E[i] & m);
                         }
+                    } else if (c == 16u && elen == 2) {
+                        // a break right after the word, between two words: its '\r' is byte 16, in the slot (item_range)
+                        ok = ((y4 >> sh) & 0xffu) == 0x0du;
                     }
                     // conservative layout check: every kept byte must lie in 0x40..0x7f (letters)
                     const uint32_t all = V[0] & V[1] & V[2] & V[3], hi = V[0] | V[1] | V[2] | V[3];
