@@ -49,6 +49,9 @@ namespace fxg {
 constexpr int REGION   = 2048;            // bytes per warp
 constexpr int SEGCAP   = 128;             // newline-list entries kept per region (lines >= 16 B on average)
 constexpr int MARK_WARPS = 8;             // warps per CTA of the mark / rows kernels
+// FASTA mark: each warp prefetches into L2 the region this many regions ahead, a little more than one wave of the grid
+// (132 SMs x 6 CTAs x 8 warps = 6336 regions on an H100), so the warps of the next wave find their bytes in L2
+constexpr int64_t MARK_AHEAD = 8192;
 constexpr int PS_THREADS = 256, PS_PER_THREAD = 16, PS_BLOCK = PS_THREADS * PS_PER_THREAD;   // regions per prefix block
 constexpr int64_t NOPOS = INT64_MIN / 4;
 constexpr uint32_t E_POS = 0x07ffu, E_CR = 1u << 14, E_HDR = 1u << 15;
@@ -121,6 +124,10 @@ struct ScanParams {
                             // (r02 ncu: 1 GB of DRAM writes per 5 GB FASTQ came from that copy alone)
 };
 
+// the REGION bytes at p (16-byte aligned) into L2, one bulk request without registers held
+__device__ __forceinline__ void prefetch_l2(const uint8_t *p) {
+    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" :: "l"(p), "n"(REGION) : "memory");
+}
 __device__ __forceinline__ uint4 ld_stream16(const uint8_t *p) {
     uint4 v;
     asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0, %1, %2, %3}, [%4];"
@@ -139,8 +146,9 @@ __device__ __forceinline__ uint4 ld_stream16(const uint8_t *p) {
 // the per-byte flags are packed into a position-ordered 64-bit mask by integer multiply-adds -- work for the FMA pipe
 // where the r01 code kept the ALU pipe busy.  V = 1 tests every 16-byte chunk where it was loaded.
 // One region per warp: a warp that also had the next region's loads in flight was slower (2, 4, 8 regions at 4 or 5
-// CTAs per SM for the extra registers) than one region per warp at 6 CTAs per SM; the kernel is bound by instruction
-// issue, not by latency.
+// CTAs per SM for the extra registers) than one region per warp at 6 CTAs per SM.  The kernel is not bound by
+// instruction issue: skipping the shared-memory copy and pass 2 for headerless regions did not make it faster
+// (DESIGN.md section 3, the read floor of mark's shape).
 __device__ __forceinline__ uint32_t swz_unit(uint32_t u) { return u ^ ((u >> 3) & 7u); }
 // byte p (0 .. REGION-1) of a region held in swizzled (V = 2) or linear (V = 1) shared memory
 template <int V>
@@ -167,6 +175,8 @@ __global__ void __launch_bounds__(MARK_WARPS * 32, FXG_MARK_MINB) mark_kernel(co
         const uint8_t *src = file + base + lane * 16;
 #pragma unroll
         for (int j = 0; j < 4; ++j) v[j] = ld_stream16(src + j * 512);
+        // more of the file in flight than the registers of 48 warps per SM hold, at no register cost
+        if (MODE == 0 && lane == 0 && base + (MARK_AHEAD + 1) * REGION <= n) prefetch_l2(file + base + MARK_AHEAD * REGION);
     } else {
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
