@@ -22,6 +22,14 @@ static int64_t fxo_next_line(const uint8_t *buf, int64_t n, int64_t cur, int64_t
     return n - cur;
 }
 
+/* the uniform-lines bit of a record from the scan's counters: `bad` lines differ from the first
+ * (line_len), the last one (last_len) among them or not; uniform iff no line but the last
+ * differs and the last is no longer than the first */
+static uint8_t fxo_uniform(int64_t bad, int64_t line_len, int64_t last_len) {
+    const int64_t bad_before_last = bad - (last_len != line_len ? 1 : 0);
+    return (uint8_t)(bad_before_last == 0 && last_len <= line_len);
+}
+
 /* ---- FASTA index scan -------------------------------------------------------------------
  * pyfastx_create_index, src/index.c:230-361.
  *  - position advances by len+1 per line, also for an unterminated last line (230-231),
@@ -35,12 +43,18 @@ static int64_t fxo_next_line(const uint8_t *buf, int64_t n, int64_t cur, int64_t
  *  - norm = bad <= 1 (237, 342).  The last record is always flushed (341-357).
  * Returns the number of rows (also when it exceeds cap; only cap rows are stored).
  * *no_header is set when the input never had a header line: the reference then still
- * writes one row (start = 0, NULL name); we return that row with nlen = -1. */
+ * writes one row (start = 0, NULL name); we return that row with nlen = -1.
+ *
+ * pad[0] is not reference behaviour: it is the "uniform lines" bit the GPU scan keeps for its own
+ * kernels (they may index such a record with the slice formula).  With L_1 .. L_k the record's
+ * sequence-line lengths counted as len + 1 (the unterminated last line of the file included), the
+ * record is uniform iff L_1 = ... = L_{k-1} and L_k <= L_1 (always for k <= 1).  pad[1..5] stay 0. */
 int64_t fxo_fasta_scan(const uint8_t *buf, int64_t n, int full_name,
                        fxo_fasta_row *rows, int64_t cap,
                        int64_t *total_slen, int *no_header) {
     int64_t cur = 0, next = 0, len;
     int64_t position = 0, start = 0, seq_len = 0, line_len = 0, bad = 0, total = 0;
+    int64_t last_len = 0;   /* len + 1 of the record's latest sequence line (0: none yet) */
     int64_t nrows = 0;
     int32_t dlen = 0, nlen = -1;
     int elen = 1;
@@ -61,12 +75,13 @@ int64_t fxo_fasta_scan(const uint8_t *buf, int64_t n, int full_name,
                     r->norm = (uint8_t)(bad > 1 ? 0 : 1);
                     r->dlen = dlen;
                     r->nlen = nlen;
+                    r->pad[0] = fxo_uniform(bad, line_len, last_len);
                 }
                 ++nrows;
                 total += seq_len;
             }
             start = position;
-            seq_len = 0; line_len = 0; bad = 0;
+            seq_len = 0; line_len = 0; bad = 0; last_len = 0;
             elen = (line[len - 1] == '\r') ? 2 : 1;
             dlen = (int32_t)(len - elen);
             if (full_name) {
@@ -80,6 +95,7 @@ int64_t fxo_fasta_scan(const uint8_t *buf, int64_t n, int full_name,
             int64_t temp = len + 1;
             if (line_len > 0 && line_len != temp) ++bad;
             if (line_len == 0) line_len = temp;
+            last_len = temp;
             seq_len += len - elen + 1;
         }
         cur = next;
@@ -96,6 +112,7 @@ int64_t fxo_fasta_scan(const uint8_t *buf, int64_t n, int full_name,
         r->norm = (uint8_t)(bad > 1 ? 0 : 1);
         r->dlen = dlen;
         r->nlen = nlen;
+        r->pad[0] = fxo_uniform(bad, line_len, last_len);
     }
     if (no_header) *no_header = (start == 0);
     ++nrows;

@@ -27,7 +27,7 @@ typedef struct fxo_fasta_row {
     int32_t nlen;   /* chrom name length (index.c:282-301)                              */
     uint8_t elen;   /* 1 = \n, 2 = \r\n, decided on the header line (index.c:267-269)   */
     uint8_t norm;   /* <=1 line differing from the first one (index.c:237,342)          */
-    uint8_t pad[6];
+    uint8_t pad[6]; /* pad[0]: uniform lines, not in the reference (fxo_fasta_scan)     */
 } fxo_fasta_row;    /* 48 bytes; name bytes start at boff - elen - dlen                 */
 
 /* One `read` table row (reference DDL: src/fastq.c:29-37). */

@@ -136,12 +136,13 @@ def mixed_fasta(seed=0):
 
 
 def record_lines(data, row):
-    """lengths of the sequence lines of one record (end of line included), from the bytes"""
+    """lengths of the sequence lines of one record (end of line included), from the bytes; the unterminated last line
+    of a file counts its virtual newline, as the scan does (blen already runs one past the end of the file there)"""
     a = np.frombuffer(data, np.uint8)
     b0 = int(row["boff"])
-    b1 = min(b0 + int(row["blen"]), a.size)
-    nl = np.flatnonzero(a[b0:b1] == 10) + 1
-    ends = np.concatenate([nl, [b1 - b0]]) if (nl.size == 0 or nl[-1] != b1 - b0) else nl
+    blen = int(row["blen"])
+    nl = np.flatnonzero(a[b0:min(b0 + blen, a.size)] == 10) + 1
+    ends = np.concatenate([nl, [blen]]) if (nl.size == 0 or nl[-1] != blen) else nl
     return np.diff(np.concatenate([[0], ends]))
 
 

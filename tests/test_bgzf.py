@@ -122,7 +122,7 @@ def test_fasta_on_bgzf_equals_plain(tmp_path):
     fa, fb = pyfastx.Fasta(str(plain)), pyfastx.Fasta(str(bg))
     assert fb.is_gzip and fb._st.bgzf_members > 1 and not fa.is_gzip
     assert fa.keys() == fb.keys() and len(fa) == 300
-    for fld in ("boff", "blen", "slen", "llen", "dlen", "nlen", "elen", "norm"):
+    for fld in ("boff", "blen", "slen", "llen", "dlen", "nlen", "elen", "norm", "pad"):
         assert np.array_equal(fa._rows[fld], fb._rows[fld])
     rid, s, e, minus = synth.random_queries(fa._rows["slen"], 3000, seed=124)
     a, oa, _ = fa.extract(rid, s, e, minus)

@@ -46,6 +46,8 @@ def test_c2_fasta_10gb_rows_and_extraction(eng):
     assert np.array_equal(rows["llen"], np.minimum(lengths, 80) + 1)
     assert (rows["elen"] == 1).all() and (rows["norm"] == 1).all()
     assert np.array_equal(rows["dlen"], hdr - 2) and np.array_equal(rows["nlen"], 3 + _ndig(idx))
+    # 80-column lines, the last one no longer: every record has uniform lines (pad[0]), the other pad bytes stay 0
+    assert (rows["pad"][:, 0] == 1).all() and (rows["pad"][:, 1:] == 0).all()
     # extraction round trips on 2M random windows of mixed length
     rid, s, e, minus = synth.random_queries(lengths, 2_000_000, seed=123, mixed=True)
     fl_plus = np.zeros(rid.size, dtype=np.int32)

@@ -178,7 +178,7 @@ def fastq_sets(tmp_path_factory):
 def test_layout_rows(fasta_set, fastq_sets):
     """the scan gives each record the intended layout: norm and the uniform-line flag (pad[0] & 1)"""
     fa, orows = fasta_set["fa"], fasta_set["orows"]
-    for f in ("boff", "blen", "slen", "llen", "elen", "norm", "dlen", "nlen"):
+    for f in ("boff", "blen", "slen", "llen", "elen", "norm", "dlen", "nlen", "pad"):
         assert np.array_equal(fa._rows[f], orows[f]), f
     for i, lay in enumerate(fasta_set["layouts"]):
         assert fa[i].name == lay["name"] and len(fa[i]) == lay["slen"]

@@ -171,7 +171,7 @@ def test_sharded_host_logic_gloo(world):
     got = np.concatenate([p[0] for p in fa_parts])
     assert n_total == len(exp) and sum(p[1] for p in fa_parts) == exp_total
     assert base == np.concatenate([[0], np.cumsum([len(p[0]) for p in fa_parts])[:-1]]).tolist()
-    for f in ("boff", "blen", "slen", "llen", "dlen", "nlen", "elen", "norm"):
+    for f in ("boff", "blen", "slen", "llen", "dlen", "nlen", "elen", "norm", "pad"):
         assert np.array_equal(got[f], exp[f]), f
     qexp, qsize, qlines = fxo.fastq_scan(fq)
     qgot = np.concatenate([p[0] for p in fq_parts])

@@ -45,8 +45,6 @@ def tmpd(tmp_path_factory):
 def assert_rows_equal(got, exp, what=""):
     assert got.shape == exp.shape, (what, got.shape, exp.shape)
     for f in exp.dtype.names:
-        if f == "pad":
-            continue
         bad = np.nonzero(got[f] != exp[f])[0]
         assert bad.size == 0, "%s: field %s differs at rows %s: got %s expected %s" % (
             what, f, bad[:5], got[f][bad[:5]], exp[f][bad[:5]])
@@ -253,8 +251,7 @@ def test_loopback_layouts(name, engs, stager, tmpd):
     res, infos = S.emulate(engs, lay.pts, lay.mode, path=path, stager=stager, full_name=lay.full_name, C=BIG_BASE)
     rows = check_emulation(lay, lay.pts, res, infos, BIG_BASE, (name, "cuts + 2^33"))
     for f in rows.dtype.names:
-        if f != "pad":
-            assert np.array_equal(rows[f] - (BIG_BASE if f in OFFSET_FIELDS[lay.mode] else 0), base_rows[f]), f
+        assert np.array_equal(rows[f] - (BIG_BASE if f in OFFSET_FIELDS[lay.mode] else 0), base_rows[f]), f
     for world in WORLDS:
         pts = shard.split_points_path(path, world, lay.mode == 0)
         res, infos = S.emulate(engs, pts, lay.mode, path=path, stager=stager, full_name=lay.full_name)
